@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- images/sec of the VisualCloze denoising hot path on B200 (BASELINE.json metric).
+"""bench.py -- images/sec of the VisualCloze denoising hot path on an H100 (BASELINE.json metric).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload B|A|Bp|D|E]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload B|A|Bp|D|E] [--dump-outputs DIR]
 
 One "step" = one image of the workload: the flow-matching Euler loop over the FLUX-DiT (30 time points = 29 model
 evaluations for the 384 grid 2x3 layout, SURVEY.md section 8) plus the VAE decode of the query row, on synthetic
@@ -11,7 +11,7 @@ inputs of the reference's shapes with random-init weights of the reference's geo
   e2e     the same through the public API with HOST (pinned) buffers: H2D of the step's inputs and D2H of the
           result inside the timed region
   roofline / roofline_attention   achieved TFLOP/s of the GEMM / attention kernels (algorithmic FLOPs over the sum of
-          their launch durations, CUDA events around every launch of one instrumented image) vs the measured peak
+          their launch durations, CUDA events around every launch of one instrumented image) vs the peak (see peaks())
   cpu_baseline   the CPU oracle port (the reference's algorithm, un-merged LoRA, bf16 autocast semantics) timed on
           the host cores on a bounded sample (1 double + 1 single block at full width and full token count),
           extrapolated to images/sec -- a reported baseline, not the target.
@@ -20,9 +20,12 @@ inputs of the reference's shapes with random-init weights of the reference's geo
 SingleStreamBlock of models/modules/layers.py with LoRA r=256, bf16 autocast, attention through SDPA because flash-attn is
 CUDA-only) on the host cores -- `cpu_baseline.kind` "reference"; the restated oracle ("port") only if oracle/_ref is absent.
 
-With N > 1 GPUs the default line is replica throughput (weak scaling, the contract's line); after it the same process group
-runs the sequence-parallel single-image mode for a few images and reports it under `extra.sp` (strong scaling, one image over
-the N GPUs), so the driver's scaling record also carries the NVLink path.
+With N > 1 GPUs the default line is replica throughput (weak scaling); after it the same process group runs the
+sequence-parallel single-image mode for a few images and reports it under `extra.sp` (strong scaling, one image over the N
+GPUs), so a scaling record also carries the NVLink path.
+
+`--dump-outputs DIR` writes what the last timed step returned -- the decoded query row (`image.npy`) and the final latent it was
+decoded from (`latent.npy`), float32 -- so that two builds can be compared output for output: the inputs are seeded.
 """
 from __future__ import annotations
 
@@ -56,7 +59,8 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf=d["bf16_tflops_sustained"], src="measured")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf=1400.0, src="fallback")
+    # NVIDIA's data sheet for the H100 SXM at 700 W: 3.35 TB/s HBM3, 989 TFLOP/s dense bf16 -- denominators, not measurements
+    return dict(hbm=3350.0, tf_burst=989.0, tf=989.0, src="H100 SXM data sheet")
 
 
 # ------------------------------------------------------------------------------------------------------
@@ -257,8 +261,10 @@ def main():
     ap.add_argument("--precision", default="bf16", choices=["bf16", "fp8", "fp8_all"],
                     help="bf16 = the reference's numerics (the headline); fp8 = opt-in e4m3 projections for the LayerNorm-fed Linears "
                          "(a separate line with its own tolerance contract, never the headline)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the arrays the last timed step returned as DIR/<name>.npy (float32)")
     ap.add_argument("--mode", default="replicas", choices=["replicas", "sp"],
-                    help="N>1: 'replicas' = one image per GPU (throughput, weak scaling; the default and the contract's line); "
+                    help="N>1: 'replicas' = one image per GPU (throughput, weak scaling; the default); "
                          "'sp' = ONE image sharded by token rows over the N GPUs (latency, strong scaling; SURVEY.md 8f-2)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
@@ -268,7 +274,7 @@ def main():
     nfe = num_steps - 1
     config = {"workload": f"{args.workload}: {desc}", "grid": f"{gh}x{gw}", "resolution": res, "num_steps": num_steps,
               "nfe": nfe, "batch_per_gpu": 1, "parallelism": f"replicas x{world} (no per-step collective; all_gather of result tiles)",
-              "lora": "merged r=256", "l2": "per-evaluation working set is 24 GB of weights >> 126 MB L2 (no flush needed)"}
+              "lora": "merged r=256", "l2": "per-evaluation working set is 24 GB of weights >> 50 MB L2 (no flush needed)"}
 
     sp_mode = args.mode == "sp" and world > 1
     if sp_mode:
@@ -293,13 +299,13 @@ def main():
 
     # ---------------- our arm ----------------
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py --impl ours needs a B200: the hot path has no CPU fallback")
+        raise SystemExit("bench.py --impl ours needs an H100: the hot path has no CPU fallback")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     if world > 1:
         import datetime
         import torch.distributed as dist
-        dist.init_process_group("nccl", device_id=dev, timeout=datetime.timedelta(minutes=5))   # a stuck rank ends the run, not the lease
+        dist.init_process_group("nccl", device_id=dev, timeout=datetime.timedelta(minutes=5))   # a stuck rank ends the run
     from visualcloze_b200 import _lib, model as M, transport as T
     lib = _lib.lib()
     with torch.device(dev):
@@ -310,7 +316,7 @@ def main():
         config["precision"] = (("fp8: qkv / mlp.0 / linear1 (58 % of the GEMM FLOPs)" if args.precision == "fp8" else
                                 "fp8_all: every Linear of the blocks (qkv, proj, mlp.0, mlp.2, linear1, linear2; inputs of the gated-residual ones "
                                 "quantised row-wise by quantize_rows_e4m3_kernel, booked under other_ms)") +
-                               " on e4m3 operands (tcgen05 kind::f8f6f4, per-row activation and per-channel weight scales); everything else bf16.  "
+                               " on e4m3 operands (wgmma e4m3, per-row activation and per-channel weight scales); everything else bf16.  "
                                "NOT the reference's numerics: tests/test_fp8_gpu.py")
     model.engine()
     decoder = None
@@ -344,8 +350,12 @@ def main():
             return out
         return tile
 
+    last = {}
+
     def step_resident():
-        return finish(fn(x_d, model.forward, kw_d)[-1])
+        last["latent"] = fn(x_d, model.forward, kw_d)[-1]
+        last["image"] = finish(last["latent"])
+        return last["image"]
 
     def step_e2e():
         x = x_h.to(dev, non_blocking=True)
@@ -374,6 +384,11 @@ def main():
     lib.vcb_reset_launch_count()
     ms = timed(step_resident, args.steps)
     launches = lib.vcb_launch_count()
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, t in last.items():
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), t.float().cpu().numpy())
     clk = clocks.stop() if clocks else None
     step_e2e()
     ms_e2e = timed(step_e2e, args.steps)
@@ -427,7 +442,7 @@ def main():
                         "gemm_ms": cat_s["gemm"][0], "attention_ms": cat_s["attention"][0], "ln_modulate_ms": cat_s["ln_modulate"][0],
                         "barrier_and_other_ms": cat_s["other"][0], "vae_ms": cat_s["vae_conv3x3"][0] + cat_s["vae_elementwise"][0],
                         "nvlink_bytes_per_eval_per_rank": int(sent),
-                        "note": "ONE image, token rows sharded over the GPUs; q/k/v and attention-output all-to-alls are TMA tile stores into "
+                        "note": "ONE image, token rows sharded over the GPUs; q/k/v and attention-output all-to-alls are stores into "
                                 "peer memory from the GEMM / attention epilogues; per-rank kernel times are rank 0's"}
             model.enable_sequence_parallel(None)
         except Exception as e:  # noqa: BLE001  (the replica line must survive a failure of the extra measurement)
@@ -442,12 +457,6 @@ def main():
     ln_bytes = nfe * 4.0 * 3072 * ((2 * 19 + 38) * (Li + Lt) + Li)
     if sp_mode:                       # rank 0's kernels did 1/W of the image's GEMM rows and attention heads
         gemm_fl, attn_fl, ln_bytes = gemm_fl / world, attn_fl / world, ln_bytes / world
-    traffic = {}
-    import glob
-    tps = sorted(glob.glob(os.path.join(REPO, "profiles", "r*_ncu_traffic.json")))   # committed ncu --set full captures, latest round
-    if tps:
-        traffic = json.load(open(tps[-1]))
-        traffic["source"] = os.path.relpath(tps[-1], REPO)
     pms = [cat[k][0] for k in _lib.PROF_CATEGORIES]
     pl = [cat[k][1] for k in _lib.PROF_CATEGORIES]
     # the GEMM category also holds the VAE decoder's 1x1 convolutions / mid-attention GEMMs (M = pixels): split them off by shape
@@ -466,7 +475,7 @@ def main():
         elif r.category == 4:
             conv_fl += 2.0 * i[0] * i[1] * i[2]; conv_ms += r.ms
     shape_rows = [{"M": k[0], "N": k[1], "K": k[2], "epilogue": EPI.get(k[3], str(k[3])), "block_n": k[4], "cta_group": k[5], "launches": v[0],
-                   "avg_us": 1e3 * v[1] / v[0], "tflops": v[2] / (v[1] / v[0]) / 1e9, "frac_of_sustained_peak": v[2] / (v[1] / v[0]) / 1e9 / pk["tf"],
+                   "avg_us": 1e3 * v[1] / v[0], "tflops": v[2] / (v[1] / v[0]) / 1e9, "frac_of_peak": v[2] / (v[1] / v[0]) / 1e9 / pk["tf"],
                    "share_of_gemm_time": v[1] / max(pms[0], 1e-9)}
                   for k, v in sorted(shapes.items(), key=lambda kv: -kv[1][1]) if v[1] > 0.002 * pms[0]]
     dit_gemm_ms = pms[0] - vae_gemm_ms
@@ -480,25 +489,24 @@ def main():
         "gpu_launches": int(launches),
         "e2e": {"value": jobs * args.steps / (ms_e2e / 1000.0), "unit": "images/s", "h2d_bytes_per_step": int(h2d),
                 "d2h_bytes_per_step": int(d2h)},
-        "roofline": {"kernel": "gemm_bf16_tcgen05_kernel (all fused-epilogue GEMMs of the FLUX-DiT for one image)", "bound": "tensor",
+        "roofline": {"kernel": "gemm_wgmma_kernel (all fused-epilogue GEMMs of the FLUX-DiT for one image)", "bound": "tensor",
                      "achieved": gemm_fl / (dit_gemm_ms / 1000.0) / 1e12, "peak": pk["tf"], "unit": "TFLOP/s",
                      "frac": gemm_fl / (dit_gemm_ms / 1000.0) / 1e12 / pk["tf"],
-                     "traffic": traffic.get("gemm", {}).get("avg_dram_bytes_per_launch"), "traffic_source": traffic.get("source"), "peak_source": pk["src"] + " sustained",
+                     "peak_source": pk["src"],
                      "launches": int(pl[0]), "avg_launch_ms": pms[0] / max(1, pl[0]), "flops_per_image": gemm_fl,
                      **({"peak_note": ("58 % of these FLOPs" if args.precision == "fp8" else "the blocks' FLOPs (all but img_in / final / modulation)") +
                                       " ran on e4m3 operands, whose dense peak is 2x the bf16 peak used as the denominator here"}
                         if args.precision != "bf16" else {})},
-        "roofline_attention": {"kernel": "attn_fwd4_tcgen05_kernel (persistent schedule; fixed-reference softmax where the block's QK-norm bound applies)",
+        "roofline_attention": {"kernel": "attn_fwd_wgmma_kernel (fixed-reference softmax where the block's QK-norm bound applies)",
                                "bound": "tensor", "achieved": attn_fl / (pms[1] / 1000.0) / 1e12,
                                "peak": pk["tf"], "unit": "TFLOP/s", "frac": attn_fl / (pms[1] / 1000.0) / 1e12 / pk["tf"],
-                               "launches": int(pl[1]), "avg_launch_ms": pms[1] / max(1, pl[1]), "softmax_variant_per_block": variants,
-                               "traffic": traffic.get("attention", {}).get("avg_dram_bytes_per_launch")},
+                               "launches": int(pl[1]), "avg_launch_ms": pms[1] / max(1, pl[1]), "softmax_variant_per_block": variants},
         "roofline_ln_modulate": {"kernel": "ln_modulate_stats_kernel (statistics from the producing GEMM's epilogue; ln_modulate2_kernel for the first LayerNorm of an evaluation)"
                                  if args.precision == "bf16" else "ln_modulate_fp8_kernel (e4m3 rows + per-row scales) + ln_modulate2_kernel", "bound": "hbm", "unit": "GB/s", "peak": pk["hbm"],
                                  "achieved": ln_bytes / (pms[2] / 1000.0) / 1e9, "frac": ln_bytes / (pms[2] / 1000.0) / 1e9 / pk["hbm"],
                                  "launches": int(pl[2]), "avg_launch_ms": pms[2] / max(1, pl[2]),
-                                 "note": "algorithmic bytes = read + write of the normalised rows; CUDA events around a ~14 us kernel (ncu: 14.0 us, profiles/r02_summary.md) include ~4 us of launch latency"},
-        "roofline_vae": {"kernel": "gemm_bf16_tcgen05_kernel<A_CONV3X3> (implicit-GEMM 3x3 convolutions of the decoder, query row)",
+                                 "note": "algorithmic bytes = read + write of the normalised rows; CUDA events around a kernel this short include its launch latency"},
+        "roofline_vae": {"kernel": "gemm_wgmma_kernel<A_CONV3X3> (implicit-GEMM 3x3 convolutions of the decoder, query row)",
                          "bound": "tensor", "unit": "TFLOP/s", "peak": pk["tf"], "achieved": conv_fl / max(conv_ms, 1e-9) / 1e9,
                          "frac": conv_fl / max(conv_ms, 1e-9) / 1e9 / pk["tf"], "launches": int(pl[4]), "conv_ms": conv_ms,
                          "conv_flops": conv_fl, "other_gemm_ms": vae_gemm_ms, "other_gemm_flops": vae_gemm_fl,

@@ -1,4 +1,4 @@
-/* vcb200.h -- C ABI of libvcb200.so: the B200-native VisualCloze denoising hot path.
+/* vcb200.h -- C ABI of libvcb200.so: the H100-native (sm_90a) VisualCloze denoising hot path.
  *
  * The reference (lzyhha/VisualCloze) is pure Python and has no FFI layer; its boundary for this path is a set
  * of Python call signatures (SURVEY.md 8b).  Each entry point below names the reference code it replaces
@@ -81,7 +81,7 @@ typedef struct vcb_gemm_args {
     void* out2; int64_t ldo2; int32_t out2_col_offset;
     /* tuning: 0 = library heuristic */
     int32_t block_n;                 /* 64 / 128 / 192 / 256 */
-    int32_t cta_group;               /* 1 or 2 (CTA pair, tcgen05 cta_group::2) */
+    int32_t cta_group;               /* 1 or 2 (2-CTA cluster on a 256-row tile, multicast B) */
     /* sequence-parallel head routing (VCB_EPI_QKV / VCB_EPI_LINEAR1, one sample; sp_world <= 1 = off): token rows are
        sharded over sp_world ranks and attention heads over the same ranks, so the epilogue stores the q/k/v columns of
        head h directly into rank h / (heads / sp_world)'s peer-mapped buffer sp_out[rank] -- layout
@@ -95,7 +95,7 @@ typedef struct vcb_gemm_args {
     void* row_stats;
     /* FP8 operands (opt-in; VCB_EPI_BIAS / BIAS_GELU / QKV / LINEAR1, plain matrices): operand_dtype = VCB_DTYPE_E4M3 makes A
        and W e4m3 bytes (lda / ldw / a_batch_stride in elements = bytes, multiples of 16), multiplied on the tensor cores with
-       tcgen05.mma kind::f8f6f4; the fp32 accumulator is rescaled by a_scale[mapped OUTPUT row] * w_scale[column] before the
+       wgmma e4m3 x e4m3; the fp32 accumulator is rescaled by a_scale[mapped OUTPUT row] * w_scale[column] before the
        bias (per-row activation scales as written by vcb_ln_modulate_fp8, per-output-channel weight scales; NULL = 1). */
     int32_t operand_dtype;           /* VCB_DTYPE_BF16 (0) or VCB_DTYPE_E4M3 (1) */
     const float* a_scale;
@@ -111,7 +111,7 @@ int vcb_gemm_bf16(const vcb_gemm_args* args, void* stream);
 int vcb_gemm_bf16_grouped(const vcb_gemm_args* args0, const vcb_gemm_args* args1, void* stream);
 
 /* ---- 3x3 convolution, stride 1, zero padding 1, NHWC bf16 (models/modules/autoencoder.py:63,65,101,239,258) ------
- * Implicit GEMM on the tcgen05 kernel without im2col: each k-block is one 4-D TMA box of a 16x8 pixel patch at the
+ * Implicit GEMM on the wgmma kernel without im2col: each k-block is one 4-D TMA box of a 16x8 pixel patch at the
  * filter tap's shift, zero-filled outside the image.  x [n,H,W,cin], w [cout, 3,3,cin] (tap-major, channels last),
  * out [n,H/stride,W/stride,cout]; res (optional, same shape as out): out = bf16(res + bf16(conv + bias)).
  * stride 1: zero padding 1 all round.  stride 2: the encoder's Downsample (autoencoder.py:85-95): pad right/bottom by 1,
@@ -280,7 +280,7 @@ void vcb_flux_destroy(vcb_flux* f);
  * checkpoint whose QK-norm scales leave the safe range gets anyway; used to measure that path on any weights */
 int  vcb_flux_use_score_bounds(vcb_flux* f, int32_t enable);
 /* opt-in FP8 (e4m3) projections: the Linears fed by an AdaLN LayerNorm (double blocks: img/txt qkv and mlp.0; single blocks:
- * linear1 -- 58 % of the step's GEMM FLOPs) run on tcgen05.mma kind::f8f6f4 with per-row activation scales (written by the
+ * linear1 -- 58 % of the step's GEMM FLOPs) run on e4m3 wgmma with per-row activation scales (written by the
  * LayerNorm kernel) and per-output-channel weight scales; everything else stays bf16.  Needs the w8 / w8_scale members of those
  * weights.  level 2 (VCB_FP8_ALL_LINEARS) adds the gated-residual Linears (attn.proj, mlp.2, linear2 -- all of the blocks' GEMM
  * FLOPs): their bf16 inputs (attention output, GELU output) are quantised row-wise by vcb_quantize_rows_e4m3 first.
@@ -334,7 +334,7 @@ int vcb_flux_sp_attach(vcb_flux* f, int32_t world, int32_t rank, void* const* qk
                        int32_t* err, int32_t timeout_ms);
 
 /* ---- VAE decoder (models/modules/autoencoder.py:183-259, 307-309; the pipeline's AutoencoderKL.decode, visualcloze.py:430)
- * NHWC bf16 activations; 3x3 convs as implicit tcgen05 GEMMs, GroupNorm(32)+swish, nearest-2x upsampling and the
+ * NHWC bf16 activations; 3x3 convs as implicit wgmma GEMMs, GroupNorm(32)+swish, nearest-2x upsampling and the
  * single-head mid-block attention as HBM-bound kernels.  Conv weights are [cout, 3, 3, cin_padded] bf16 (tap-major,
  * channels last, cin padded to a multiple of 64, cout of conv_out padded to 8), 1x1 convs [cout, cin]; biases and
  * GroupNorm affine parameters fp32. */
@@ -393,12 +393,12 @@ int64_t vcb_vae_enc_workspace_bytes(const vcb_vae_enc* e, int32_t n, int32_t H, 
 int vcb_vae_encode(vcb_vae_enc* e, void* workspace, int64_t workspace_bytes, const float* image, int32_t n, int32_t H,
                    int32_t W, const float* noise, void* tokens, float* moments, void* stream);
 
-/* ---- test hook: one 128x128x(16*ksteps) tcgen05 MMA with caller-chosen descriptor fields -------------------
- * Used by tests/ to pin the smem/TMEM operand layouts the kernels rely on.  a: [128, K] bf16 (K-major),
+/* ---- test hook: one 128x128x(16*ksteps) wgmma tile with caller-chosen descriptor fields -------------------
+ * Used by tests/ to pin the shared-memory / register operand layouts the kernels rely on.  a: [128, K] bf16 (K-major),
  * b: B operand, either [128(N), K] K-major (b_mn_major=0) or [K, 128(N)] N-contiguous (b_mn_major=1);
- * a_from_tmem: stage A through TMEM (tcgen05.st) instead of smem.  out: [128,128] fp32. */
+ * a_from_regs: feed A from registers (the accumulator's row layout) instead of smem.  out: [128,128] fp32. */
 int vcb_debug_umma_probe(const void* a, const void* b, float* out, int32_t ksteps, int32_t b_mn_major,
-                         int32_t a_from_tmem, uint32_t b_lbo, uint32_t b_sbo, uint32_t b_kstep_bytes, void* stream);
+                         int32_t a_from_regs, uint32_t b_lbo, uint32_t b_sbo, uint32_t b_kstep_bytes, void* stream);
 
 #ifdef __cplusplus
 }

@@ -31,6 +31,7 @@ container by ``oracle/gen_golden.py`` and committed under ``tests/golden/``.
 """
 from __future__ import annotations
 
+import collections.abc
 import math
 from dataclasses import dataclass, field
 
@@ -329,6 +330,22 @@ def flux_vec(p, cfg, timesteps, y, guidance, nm, ls):
     return vec + mlp_embedder(p, "vector_in", y, nm, ls)
 
 
+class _Fp32View(collections.abc.Mapping):
+    """The parameters in fp32, converted as they are read (a full-size model does not fit a device twice over)."""
+
+    def __init__(self, p):
+        self.p = p
+
+    def __iter__(self):
+        return iter(self.p)
+
+    def __len__(self):
+        return len(self.p)
+
+    def __getitem__(self, k):
+        return self.p[k].float()
+
+
 def flux_forward(p: dict, cfg: FluxConfig, img, img_ids, txt, txt_ids, timesteps, y,
                  txt_mask=None, img_mask=None, guidance=None, mode: str = "cuda_bf16",
                  taps: dict | None = None) -> torch.Tensor:
@@ -338,7 +355,7 @@ def flux_forward(p: dict, cfg: FluxConfig, img, img_ids, txt, txt_ids, timesteps
     nm = Numerics(mode)
     ls = cfg.lora_scale
     if mode == "fp32":
-        p = {k: v.float() for k, v in p.items()}
+        p = _Fp32View(p)
         img, txt, y = img.float(), txt.float(), y.float()
         guidance = None if guidance is None else guidance.float()
     img = lora_linear(p, "img_in", img, nm, ls)

@@ -1,7 +1,7 @@
 """Context number, NOT part of the product or of bench.py: the reference's algorithm (oracle port, un-merged LoRA r=256,
 bf16 autocast semantics) executed EAGERLY ON THE GPU with library kernels -- cuBLAS GEMMs, ATen elementwise ops and the
 same flash-attn 2.x kernel the reference calls (models/math.py:85-95) -- on the cfg-B shapes.  It approximates what the
-unmodified reference costs per model evaluation on this B200 (the reference itself cannot travel to the GPU box).
+unmodified reference costs per model evaluation on this H100 (the reference itself is not part of this repository).
 
     python tests/perf_reference_gpu.py [n_double n_single]      -> one JSON line, extrapolated to 19 + 38 blocks
 """

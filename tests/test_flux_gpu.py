@@ -1,4 +1,4 @@
-"""Model-level parity on the B200: Flux.forward and the Euler sampler through the reference-shaped Python API
+"""Model-level parity on the H100: Flux.forward and the Euler sampler through the reference-shaped Python API
 (visualcloze_b200.model / transport -> libvcb200.so) against the CPU oracle and the reference-generated goldens.
 
 Tolerances (SURVEY.md 8c; reference-vs-reference noise, FA2 vs SDPA and merged vs un-merged LoRA, is ~1e-2):

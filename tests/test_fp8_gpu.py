@@ -4,7 +4,7 @@ The fp8 path is NOT the reference's numerics (the reference computes every Linea
 tensor-bound at ~0.8 of the bf16 peak and e4m3 operands double that peak for the 58 % of GEMM FLOPs whose A operand comes out of
 an AdaLN LayerNorm (SURVEY.md 8f-3).  Two kinds of checks:
 
-  * kernels: the fp8 GEMM (tcgen05.mma kind::f8f6f4, per-row x per-channel rescale, every epilogue it supports) against an fp32
+  * kernels: the fp8 GEMM (wgmma e4m3, per-row x per-channel rescale, every epilogue it supports) against an fp32
     matmul of the DEQUANTISED operands -- this isolates the kernel from the quantisation error, tolerance = the bf16 kernels';
     the fp8 LayerNorm against quantising the bf16 LayerNorm kernel's output in torch (scales exact, bytes within 1 e4m3 ulp);
     the row quantiser of level 2 ("fp8_all": attn.proj / mlp.2 / linear2 too) bit for bit against the same rule in torch;

@@ -1,4 +1,4 @@
-"""Parity at BASELINE.json's REAL sizes on the B200, against (a) the UNMODIFIED reference modules of ``oracle/_ref`` executed
+"""Parity at BASELINE.json's REAL sizes on the H100, against (a) the UNMODIFIED reference modules of ``oracle/_ref`` executed
 under ``torch.autocast("cuda", bf16)`` with flash-attn -- the authoritative oracle of SURVEY.md 8c -- and (b) the restated
 oracle (``oracle/flux_oracle.py``, ``cuda_bf16`` mode) executed on the same GPU.
 
@@ -23,6 +23,7 @@ The forward bar is therefore: ours-vs-reference <= 2.5e-2 AND <= 1.2 x floor_mer
 formulation), and ours is no further from the fp32 truth than 1.2 x the merged oracle is.  Trajectory and PSNR keep SURVEY's
 numbers.
 """
+import collections.abc
 import dataclasses
 import json
 import math
@@ -46,6 +47,34 @@ def _record(key, **vals):
     print(f"[fullsize] {key}: " + ", ".join(f"{k}={v:.3e}" if isinstance(v, float) else f"{k}={v}" for k, v in vals.items()))
 
 
+class _MergedView(collections.abc.Mapping):
+    """The state dict with LoRA merged, formed exactly as the engine's weight packing states it (engine.py::_linear): fp32 W + s B A,
+    one bf16 rounding.  Each entry is formed when it is read: a second resident copy of the 24 GB of weights would not fit next to
+    the model on an 80 GB device."""
+
+    def __init__(self, sd):
+        self.sd = sd
+        self.keys_ = [k for k in sd if ".lora_" not in k]
+
+    def __iter__(self):
+        return iter(self.keys_)
+
+    def __len__(self):
+        return len(self.keys_)
+
+    def __getitem__(self, k):
+        sd = self.sd
+        if ".lora_" in k:
+            raise KeyError(k)
+        v = sd[k]
+        if k.endswith(".weight") and (k[:-7] + ".lora_A.weight") in sd:
+            n = k[:-7]
+            return (v.float() + sd[n + ".lora_B.weight"].float() @ sd[n + ".lora_A.weight"].float()).to(BF16)
+        if k.endswith(".bias") and (k[:-5] + ".lora_B.bias") in sd:
+            return (v.float() + sd[k[:-5] + ".lora_B.bias"].float()).to(BF16)
+        return v
+
+
 def _cuda(d):
     return {k: (v.cuda() if torch.is_tensor(v) else v) for k, v in d.items()}
 
@@ -65,19 +94,7 @@ def full():
     sd = dict(ours.state_dict())
     ref = rr.build_flux(dataclasses.asdict(P), 256, sd) if rr.available() else None
     cfg = fo.FluxConfig(**dataclasses.asdict(P), lora_rank=256)
-    # merged weights, formed exactly as the engine's weight packing states it (engine.py::_linear): fp32 W + s B A, one bf16 rounding
-    merged = {}
-    for k, v in sd.items():
-        if ".lora_" in k:
-            continue
-        if k.endswith(".weight") and (k[:-7] + ".lora_A.weight") in sd:
-            n = k[:-7]
-            merged[k] = (v.float() + sd[n + ".lora_B.weight"].float() @ sd[n + ".lora_A.weight"].float()).to(BF16)
-        elif k.endswith(".bias") and (k[:-5] + ".lora_B.bias") in sd:
-            merged[k] = (v.float() + sd[k[:-5] + ".lora_B.bias"].float()).to(BF16)
-        else:
-            merged[k] = v
-    return dict(ours=ours, ref=ref, sd=sd, merged=merged, cfg=cfg, fo=fo, rr=rr)
+    return dict(ours=ours, ref=ref, sd=sd, merged=_MergedView(sd), cfg=cfg, fo=fo, rr=rr)
 
 
 def _inputs(workload, seed=1234):

@@ -1,4 +1,4 @@
-"""Per-kernel parity on the B200: every test calls through the C ABI (visualcloze_b200.ops -> libvcb200.so)
+"""Per-kernel parity on the H100: every test calls through the C ABI (visualcloze_b200.ops -> libvcb200.so)
 and compares with the CPU oracle (oracle/flux_oracle.py) or, for the bare GEMM, a plain fp32 torch matmul of
 the same bf16 operands.  Tolerances are stated per test."""
 import math
@@ -34,7 +34,7 @@ def _stats(got, ref):
 
 
 # ------------------------------------------------------------------------------------------------
-# operand-layout probes (single tcgen05 MMA tile)
+# operand-layout probes (single wgmma tile)
 # ------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("ksteps", [4, 8])
 def test_probe_kmajor_ss(ops, ksteps):
@@ -57,7 +57,7 @@ def test_probe_b_mn_major(ops, ksteps):
 
 @pytest.mark.parametrize("ksteps", [4, 8])
 def test_probe_a_from_tmem(ops, ksteps):
-    """A staged in TMEM as packed bf16 pairs (the P tile of attention), B MN-major."""
+    """A fed from registers as packed bf16 pairs (the P tile of attention; the test keeps its first name), B MN-major."""
     K = 16 * ksteps
     a, b = _randn(128, K, seed=5), _randn(K, 128, seed=6)
     out = ops.umma_probe(a.cuda(), b.cuda(), ksteps, True, True, b_lbo=K * 128, b_sbo=1024, b_kstep_bytes=2048)

@@ -1,4 +1,4 @@
-"""Single-image sequence parallelism over NVLink peer memory (SURVEY.md 8f-2) -- needs >= 2 B200s on one node.
+"""Single-image sequence parallelism over NVLink peer memory (SURVEY.md 8f-2) -- needs >= 2 H100s on one node.
 
 Launches tests/sp_worker.py with one process per GPU (NCCL only for set-up and the final gather) and checks its report:
   * cudaIpc peer buffers, peer stores and the phase barrier work, and a barrier a peer never joins reports a time-out

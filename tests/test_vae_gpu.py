@@ -1,4 +1,4 @@
-"""VAE decoder parity on the B200 (autoencoder.py:183-259 via libvcb200) against the CPU oracle / reference golden.
+"""VAE decoder parity on the H100 (autoencoder.py:183-259 via libvcb200) against the CPU oracle / reference golden.
 bf16 activations vs the reference's fp32 golden: rel-L2 <= 3e-2 (the decoder is ~25 bf16 conv layers deep);
 decoded-image PSNR vs the oracle run with the same bf16 weights >= 35 dB (SURVEY.md 8c)."""
 import math

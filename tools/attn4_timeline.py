@@ -1,6 +1,6 @@
 """Where does the persistent attention kernel's time go?  Per-CTA globaltimer stamps (VCB_ATTN4_TIMELINE=1) of one launch:
 start, end of every segment.  Run twice: default (split tail) and VCB_ATTN4_NOSPLIT=1 (whole units).  Prints per-launch time of
-attn3 / attn4 and, for attn4, the distribution of per-CTA phase durations."""
+the per-tile grid / the persistent schedule and, for the latter, the distribution of per-CTA phase durations."""
 import ctypes as C
 import math
 import os

@@ -1,6 +1,6 @@
-"""Attention kernel vs the libraries on the reference's shapes (24 heads, head_dim 128, bf16), one B200.
+"""Attention kernel vs the libraries on the reference's shapes (24 heads, head_dim 128, bf16), one H100.
 
-  vcb  per-pair grid (attn3) / persistent (attn4)  x  exact online-max / fixed-reference softmax
+  vcb  per-tile grid / persistent schedule  x  exact online-max / fixed-reference softmax
   cuDNN SDPA (torch.nn.functional.scaled_dot_product_attention, cudnn backend), flash-attn 2 (what models/math.py:85 calls)
 
 CUDA events around each launch, L2 flushed between timed launches, median of 15.  Writes gpurun_out/attn_vs_libs.json.

@@ -1,4 +1,4 @@
-"""Micro-benchmarks of the hot kernels on one B200 (CUDA events, L2 flushed between timed launches).
+"""Micro-benchmarks of the hot kernels on one H100 (CUDA events, L2 flushed between timed launches).
 Prints one JSON line per case and writes gpurun_out/bench_kernels.jsonl.  Library kernels (cuBLAS via torch.matmul,
 FA2, cuDNN/flash SDPA) are timed next to ours as reference points only; they are never on the product path."""
 import json

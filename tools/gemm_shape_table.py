@@ -1,6 +1,5 @@
 """Per-shape GEMM table for the cfg-B FLUX-DiT step: ours (real fused epilogue) vs cuBLAS (torch.matmul, no epilogue) on the same
-shape, each run BACK TO BACK for ~0.6 s so the chip sits at its power cap like in the denoising loop (a burst number says little
-on a part that runs this workload at ~1.45 of 1.965 GHz).  CUDA events around the whole run; writes gpurun_out/gemm_shapes.json.
+shape, each run BACK TO BACK for ~0.6 s so the chip reaches the clocks it sustains in the denoising loop (a burst number says little).  CUDA events around the whole run; writes the table as JSON.
 cuBLAS is a reference point only -- it is never on the product path."""
 import json
 import math

@@ -1,4 +1,4 @@
-"""Time the full-size FLUX-DiT denoise loop (cfg B of SURVEY.md section 8) on one B200; dev tool, not the bench."""
+"""Time the full-size FLUX-DiT denoise loop (cfg B of SURVEY.md section 8) on one H100; dev tool, not the bench."""
 import os
 import sys
 import time

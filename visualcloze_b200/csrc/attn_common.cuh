@@ -1,5 +1,5 @@
-// attn_common.cuh -- parameters and constants shared by the joint-attention kernels (attn3_sm100.cuh: one CTA per query pair;
-// attn4_sm100.cuh: persistent schedule).
+// attn_common.cuh -- parameters and constants of the joint-attention kernel (attn_sm90.cuh: one CTA per query tile, or the
+// persistent schedule).
 //
 // Contract (models/math.py:63-99: attention -> _upad_input -> flash_attn_varlen_func -> pad_input): non-causal
 // softmax(Q K^T / sqrt(128)) V over right-padded samples, head_dim 128, bf16 in / fp32 accumulate / bf16 out.  Padding is handled
@@ -18,8 +18,8 @@ struct AttnParams {
     int out_col_offset;
     int q_col, k_col, v_col;     // column of head 0 of q / k / v inside the qkv matrix
     float scale_log2;            // head_dim^-0.5 * log2(e)
-    float fixed_max;             // > 0: upper bound of |score * scale_log2| guaranteed by the caller (attn_fwd3 kFixed)
-    // Sequence-parallel output routing (attn_fwd3 only, B == 1; sp_world <= 1 = off): query row r belongs to rank
+    float fixed_max;             // > 0: upper bound of |score * scale_log2| guaranteed by the caller (kFixed)
+    // Sequence-parallel output routing (B == 1; sp_world <= 1 = off): query row r belongs to rank
     // r / sp_rows and is stored over NVLink into that rank's peer-mapped buffer sp_out[rank] at row r % sp_rows.
     int sp_world, sp_rows;
     __nv_bfloat16* sp_out[8];

@@ -1,10 +1,10 @@
 #!/usr/bin/env bash
-# Builds visualcloze_b200/libvcb200.so in-tree for sm_100a (cross-compiles without a GPU).
+# Builds visualcloze_b200/libvcb200.so in-tree for sm_90a (cross-compiles without a GPU).
 set -euo pipefail
 HERE="$(cd "$(dirname "${BASH_SOURCE[0]}")" && pwd)"
 OUT="${HERE}/../libvcb200.so"
 NVCC="${NVCC:-/usr/local/cuda/bin/nvcc}"
-FLAGS=(-gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 --expt-relaxed-constexpr
+FLAGS=(-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 --expt-relaxed-constexpr
        -Xcompiler -fPIC -Xcompiler -Wall -shared)
 if [[ "${VCB_PTXAS_V:-0}" == "1" ]]; then FLAGS+=(-Xptxas -v); fi
 SRCS=("${HERE}/capi.cu")

@@ -8,13 +8,12 @@
 #include <mutex>
 
 #include "../../include/vcb200.h"
-#include "attn3_sm100.cuh"
-#include "attn4_sm100.cuh"
+#include "attn_sm90.cuh"
 #include "elementwise.cuh"
-#include "gemm_sm100.cuh"
+#include "gemm_sm90.cuh"
 #include "host_util.cuh"
 #include "probe.cuh"
-#include "sp_sm100.cuh"
+#include "sp_sm90.cuh"
 
 using namespace vcb;
 
@@ -23,7 +22,7 @@ using namespace vcb;
 // ------------------------------------------------------------------------------------------------
 namespace {
 
-struct Problem { CUtensorMap ta, tb; GemmParams p; CUtensorMap sp[kSpMaxRanks]; };
+struct Problem { CUtensorMap ta, tb; GemmParams p; };
 
 // stream-K scratch: one slot of 128 x 256 fp32 per CTA and one flag per CTA, per stream (launches on one stream are
 // ordered, so a single scratch per stream is enough); allocated on first use (call once before CUDA-graph capture)
@@ -43,16 +42,13 @@ inline SkScratch* sk_scratch(cudaStream_t st) {
 }
 // Stream-K policy.  VCB_STREAMK unset = auto, 0 = never, 1 = whenever feasible and the estimated saving exceeds 20 us.
 // Auto enables the tail split only when the idle part of the last wave is a large share of the WHOLE launch (>= 20 %) --
-// the few-wave GEMMs of the sequence-parallel mode (M ~ 2000: 96 pair tiles on 74 pairs).  Measured on B200 (cfg B,
-// power-capped at ~985 W): for the 3-wave GEMMs of the single-GPU path (idle share 13 %) the tail split is 1 % SLOWER end
-// to end -- idle SMs in a partial wave give their power budget to the busy ones (higher clocks), so most of the "lost"
-// time is recovered anyway, while the partial exchange costs real work.
+// the few-wave GEMMs of the sequence-parallel mode; with many waves the partial exchange costs more than the idle tail.
 inline int streamk_mode() {
     static const int m = [] { const char* e = getenv("VCB_STREAMK"); return e ? (atoi(e) ? 1 : 0) : -1; }();
     return m;
 }
-constexpr float kSkOverheadUs = 30.f;      // partial dump + fold of a split tile, waiting for the partners (measured, tools/bench_sk.py)
-// time of one output tile (us) for a configuration with the measured full-wave rate `rate` (TFLOP/s over all SMs)
+constexpr float kSkOverheadUs = 30.f;      // estimate: partial dump + fold of a split tile, waiting for the partners (tools/bench_sk.py measures it)
+// time of one output tile (us) for a configuration with the full-wave rate `rate` (TFLOP/s over all SMs)
 inline float tile_time_us(int bn, int K, float rate) { return 2.f * 128.f * bn * (float)K * (float)num_sms() / (rate * 1e6f); }
 inline bool streamk_feasible(long tiles, int slots) {
     // also with fewer tiles than CTA slots (one partial "wave"): every slot then gets an equal K range of the few tiles
@@ -72,8 +68,8 @@ template <int BN, int CG, int EPI, bool SP = false, bool FP8 = false>
 int launch_gemm_inst(const Problem& g0, const Problem& g1, float rate, cudaStream_t st) {
     const CUtensorMap& ta = g0.ta; const CUtensorMap& tb = g0.tb; const GemmParams& p = g0.p;
     using Cfg = GemmCfg<BN, CG>;
-    auto kern = gemm_bf16_tcgen05_kernel<BN, CG, EPI, A_MATRIX, SP, FP8>;
-    constexpr int kSmem = Cfg::kSmemBytes + (SP ? kSpStageBytes : 0);
+    auto kern = gemm_wgmma_kernel<BN, CG, EPI, A_MATRIX, SP, FP8>;
+    constexpr int kSmem = Cfg::kSmemBytes;
     static std::once_flag once;
     static cudaError_t attr_err = cudaSuccess;
     std::call_once(once, [&] {
@@ -93,11 +89,7 @@ int launch_gemm_inst(const Problem& g0, const Problem& g1, float rate, cudaStrea
         if (!sc) return set_error("gemm: stream-K scratch allocation failed");
         skp.ws = sc->ws; skp.flags = sc->flags; skp.epoch = ++sc->epoch; skp.enabled = 1;
     }
-    SpMapsT<SP> spm{};
-    if constexpr (SP) {
-        for (int r = 0; r < kSpMaxRanks; ++r) { spm.m[0][r] = g0.sp[r]; spm.m[1][r] = g1.sp[r]; }
-    }
-    cudaError_t e = launch_pdl(kern, dim3(clusters * CG), dim3(kGemmThreads), (size_t)kSmem, st, CG, ta, tb, p, g1.ta, g1.tb, g1.p, skp, spm);
+    cudaError_t e = launch_pdl(kern, dim3(clusters * CG), dim3(kGemmThreads), (size_t)kSmem, st, CG, ta, tb, p, g1.ta, g1.tb, g1.p, skp);
     if (e != cudaSuccess) return set_error("gemm launch (BN=%d CG=%d EPI=%d): %s", BN, CG, EPI, cudaGetErrorString(e));
     count_launch();
     return 0;
@@ -127,7 +119,7 @@ int launch_gemm_epi(int epi, const Problem& g0, const Problem& g1, float rate, c
         default: break;
     }
     if constexpr (BN % 128 == 0) {
-        const bool sp = g0.p.sp_world > 1;        // sequence-parallel: staged TMA tile stores into the owners' buffers
+        const bool sp = g0.p.sp_world > 1;        // sequence-parallel: stores through the owners' peer-mapped buffers
         if (epi == EPI_QKV) return sp ? launch_gemm_inst<BN, CG, EPI_QKV, true>(g0, g1, rate, st) : launch_gemm_inst<BN, CG, EPI_QKV>(g0, g1, rate, st);
         if (epi == EPI_LINEAR1) return sp ? launch_gemm_inst<BN, CG, EPI_LINEAR1, true>(g0, g1, rate, st) : launch_gemm_inst<BN, CG, EPI_LINEAR1>(g0, g1, rate, st);
     }
@@ -142,16 +134,17 @@ int forced_cta_group() {
     return v;
 }
 
-// Tile selection.  Cost of a configuration = (tiles per CTA slot, rounded up) x (tile width) / (measured per-SM
-// rate of that configuration, TFLOP/s on B200 at full waves, from tools/bench_kernels.py runs of round 1).  cta_group 2 pairs two
-// SMs on a 256 x BLOCK_N tile, halving B-operand smem traffic; narrow tiles win when they remove a partial wave.
+// Tile selection.  Cost of a configuration = (tiles per CTA slot, rounded up) x (tile width) / (full-wave rate of that
+// configuration, TFLOP/s over all SMs).  The rates are relative weights, not measurements: wider tiles re-read less of A per
+// FLOP, cta_group 2 pairs two SMs on a 256 x BLOCK_N tile and fetches each B tile from L2 once for both; narrow tiles win when
+// they remove a partial wave.  tools/bench_kernels.py measures the configurations.
 struct TileCfg { int cg, bn; float rate; };
-constexpr TileCfg kTileCfgs[] = {{2, 256, 1630.f}, {1, 256, 1445.f}, {1, 192, 1355.f}, {2, 192, 1250.f},
-                                 {1, 128, 970.f},  {2, 128, 950.f}};
+constexpr TileCfg kTileCfgs[] = {{1, 256, 600.f}, {2, 256, 600.f}, {1, 192, 560.f}, {2, 192, 560.f},
+                                 {1, 128, 500.f}, {2, 128, 500.f}};
 
 void pick_tile(int batch, int rows, int N, int K, bool head_structured, int want_cg, int want_bn, int* cg_out, int* bn_out,
                float* rate_out) {
-    float best_cost = -1.f, best_rate = 1630.f;
+    float best_cost = -1.f, best_rate = 600.f;
     int best_cg = 1, best_bn = 256;
     for (const TileCfg& c : kTileCfgs) {
         if (want_cg && c.cg != want_cg) continue;
@@ -251,12 +244,6 @@ int build_problem(const vcb_gemm_args* a, int bn, int cg, Problem* out) {
     if (int rc = make_tmap_3d(&out->ta, a->A, (uint64_t)a->K, (uint64_t)a->rows_per_batch, (uint64_t)batch, (uint64_t)a->lda,
                               (uint64_t)a_bstride, 128 / eb, 128, eb)) return rc;
     if (int rc = make_tmap_2d(&out->tb, a->W, (uint64_t)a->K, (uint64_t)a->N, (uint64_t)a->ldw, 128 / eb, (uint32_t)(bn / cg), eb)) return rc;
-    // sequence-parallel destinations: this problem's rows of every rank's [W * rows, 3 * hidden / W] qkv buffer
-    for (int r = 0; r < p.sp_world; ++r) {
-        const int64_t ld = 3LL * (a->hidden / a->sp_world);
-        const __nv_bfloat16* base = p.sp_out[r] + ((int64_t)a->sp_row_offset + a->out_row_offset) * ld;
-        if (int rc = make_tmap_2d(&out->sp[r], base, (uint64_t)ld, (uint64_t)a->rows_per_batch, (uint64_t)ld, 64, 32)) return rc;
-    }
     return 0;
 }
 
@@ -287,11 +274,8 @@ int gemm_dispatch(const vcb_gemm_args* a, const vcb_gemm_args* a1, void* stream)
         g1 = g0;
         g1.p = GemmParams{};            // batch == 0: no second problem
     }
-    // tile raster: M-fastest.  The N-fastest alternative (a wave = a band of A rows x all weight tiles, A evict-first, B evict-last),
-    // meant to stop linear2's three waves from re-reading A, was measured WORSE: 642 MB of DRAM traffic per launch instead of 522 MB
-    // (ncu, profiles/r02_summary.md) and the same time in the loop (GEMM 1167.1 vs 1167.3 ms per image) -- the 94 MB weight does not
-    // survive in L2 next to the streamed A, and evict-first drops A tiles before all twelve column tiles have fetched them.
-    // VCB_GEMM_RASTER=1 still selects it (A/B runs, tests).
+    // tile raster: M-fastest.  VCB_GEMM_RASTER=1 selects the N-fastest alternative (a wave = a band of A rows x all weight tiles,
+    // A evict-first, B evict-last) for A/B runs and tests.
     {
         static const int forced = [] { const char* e = getenv("VCB_GEMM_RASTER"); return e ? atoi(e) : -1; }();
         const int nf = forced > 0 ? 1 : 0;
@@ -332,13 +316,13 @@ extern "C" int vcb_gemm_bf16_grouped(const vcb_gemm_args* a0, const vcb_gemm_arg
 }
 
 // ------------------------------------------------------------------------------------------------
-// 3x3 convolution, NHWC, stride 1, zero padding 1: implicit GEMM on the same tcgen05 kernel (A_CONV3X3)
+// 3x3 convolution, NHWC, stride 1, zero padding 1: implicit GEMM on the same wgmma kernel (A_CONV3X3)
 // ------------------------------------------------------------------------------------------------
 namespace {
 template <int BN, int EPI>
 int launch_conv_inst(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t st) {
     using Cfg = GemmCfg<BN, 1>;
-    auto kern = gemm_bf16_tcgen05_kernel<BN, 1, EPI, A_CONV3X3>;
+    auto kern = gemm_wgmma_kernel<BN, 1, EPI, A_CONV3X3>;
     static std::once_flag once;
     static cudaError_t attr_err = cudaSuccess;
     std::call_once(once, [&] {
@@ -350,7 +334,7 @@ int launch_conv_inst(const CUtensorMap& ta, const CUtensorMap& tb, const GemmPar
     int grid = num_sms();
     if (tiles < grid) grid = tiles;
     GemmParams none{};
-    cudaError_t e = launch_pdl(kern, dim3(grid), dim3(kGemmThreads), (size_t)Cfg::kSmemBytes, st, 1, ta, tb, p, ta, tb, none, StreamKParams{nullptr, nullptr, 0, 0}, SpMapsT<false>{});
+    cudaError_t e = launch_pdl(kern, dim3(grid), dim3(kGemmThreads), (size_t)Cfg::kSmemBytes, st, 1, ta, tb, p, ta, tb, none, StreamKParams{nullptr, nullptr, 0, 0});
     if (e != cudaSuccess) return set_error("conv3x3 launch: %s", cudaGetErrorString(e));
     count_launch();
     return 0;
@@ -391,7 +375,7 @@ extern "C" int vcb_conv3x3_nhwc(const void* x, const void* w, const float* bias,
 // attention
 // ------------------------------------------------------------------------------------------------
 namespace {
-// workspace of the persistent attention kernel (attn4): one (O, l, m) slot and one flag per CTA, per stream; allocated on
+// workspace of the persistent attention schedule: one (O, l, m) slot and one flag per CTA, per stream; allocated on
 // first use (call once before CUDA-graph capture)
 struct AttnScratch { float* ws = nullptr; int* flags = nullptr; int epoch = 0; unsigned long long* timeline = nullptr; int last_grid = 0; };
 AttnScratch* g_last_attn_scratch = nullptr;       // debug: the scratch of the most recent persistent launch (vcb_debug_attn4_timeline)
@@ -410,11 +394,8 @@ inline AttnScratch* attn_scratch(cudaStream_t st) {
     }
     return &s;
 }
-// What VCB_ATTN_SCHED_AUTO resolves to.  Default: one CTA per query pair (attn3).  Measured on B200 (profiles/r02_attn_vs_libs.json,
-// r02_summary.md): timed alone (burst clocks) the per-pair grid is 8 - 20 % FASTER than the persistent kernel although it
-// executes 2.59 waves as 3; inside the denoising loop the two take the same time to the cycle (attention_ms x SM MHz equal within
-// 0.3 % for three schedules) -- the chip sits at its ~1 kW power cap there, idle SMs of a partial wave hand their budget to the
-// busy ones, and what is left to win is energy per FLOP, not occupancy.  VCB_ATTN_PERSIST=1 makes AUTO pick the persistent kernel.
+// What VCB_ATTN_SCHED_AUTO resolves to.  Default: one CTA per query tile; VCB_ATTN_PERSIST=1 makes AUTO pick the persistent
+// schedule (tools/bench_attn_quick.py compares the two).
 inline int attn_persist_mode() {
     static const int m = [] { const char* e = getenv("VCB_ATTN_PERSIST"); return (e && atoi(e)) ? 1 : 0; }();
     return m;
@@ -433,17 +414,9 @@ int attention_launch(const void* qkv, int64_t ld_qkv, int32_t q_col, int32_t k_c
     static std::once_flag once;
     static cudaError_t attr_err = cudaSuccess;
     std::call_once(once, [&] {
-        attr_err = cudaFuncSetAttribute(attn_fwd3_tcgen05_kernel<false, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttn3SmemBytes);
+        attr_err = cudaFuncSetAttribute(attn_fwd_wgmma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmemBytes);
         if (attr_err == cudaSuccess)
-            attr_err = cudaFuncSetAttribute(attn_fwd3_tcgen05_kernel<true, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttn3SmemBytes);
-        if (attr_err == cudaSuccess)
-            attr_err = cudaFuncSetAttribute(attn_fwd3_tcgen05_kernel<false, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttn3SmemBytes);
-        if (attr_err == cudaSuccess)
-            attr_err = cudaFuncSetAttribute(attn_fwd3_tcgen05_kernel<true, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttn3SmemBytes);
-        if (attr_err == cudaSuccess)
-            attr_err = cudaFuncSetAttribute(attn_fwd4_tcgen05_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttn4SmemBytes);
-        if (attr_err == cudaSuccess)
-            attr_err = cudaFuncSetAttribute(attn_fwd4_tcgen05_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttn4SmemBytes);
+            attr_err = cudaFuncSetAttribute(attn_fwd_wgmma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmemBytes);
     });
     if (attr_err != cudaSuccess) return set_error("cudaFuncSetAttribute(attn): %s", cudaGetErrorString(attr_err));
     CUtensorMap tm;
@@ -466,61 +439,41 @@ int attention_launch(const void* qkv, int64_t ld_qkv, int32_t q_col, int32_t k_c
         }
     }
     ProfScope prof(PROF_ATTN, stream, B, L, heads, fixed ? 1 : 0);
-    // Persistent schedule (attn4): unpadded batches with enough (query tile x key tile) work to give every SM a share of at
-    // least a few key tiles; right-padded batches, the sequence-parallel routing and the A/B variants stay on attn3.
+    // Persistent schedule: unpadded batches with enough (query tile x key tile) work to give every SM a share of at least a few
+    // key tiles; right-padded batches stay on the per-tile grid.
     const long long n_qt = (L + kAttnTile - 1) / kAttnTile;
-    const long long n_units = (long long)B * heads * ((n_qt + 1) / 2), total_steps = n_units * n_qt;
+    const long long n_units = (long long)B * heads * n_qt, total_steps = n_units * n_qt;
     int pgrid = num_sms();
     if (total_steps / pgrid < 4) pgrid = (int)(total_steps / 4 > 0 ? total_steps / 4 : 1);   // tiny problems: >= 4 key-tile steps per CTA
     // a CTA's segment list: one entry per full round + the pieces of its tail share; beyond the kernel's capacity (huge batches of
-    // short sequences) use the per-pair grid
-    // sequence-parallel routing: the persistent kernel stores O rows straight through the peer-mapped pointers (no TMA staging).
-    // Few heads per rank leave the per-pair grid far below one wave (cfg B: 96 CTAs at 4 ranks, 48 at 8) and these ranks are not
-    // power-capped.  The split costs ~20 us per launch (partial dump, fold, phase hand-over; tools/attn4_timeline.py), so it
-    // pays only when the per-pair grid would fill < 40 % of the SMs (8 ranks); measured equal at 2 ranks and at 96 CTAs.
+    // short sequences) use the per-tile grid.
+    // Sequence-parallel routing (O rows leave through the peer-mapped pointers in either schedule): few heads per rank leave the
+    // per-tile grid below one wave, and the key-tile split then fills the idle SMs; it costs a partial dump, a fold and a phase
+    // hand-over per launch (tools/attn4_timeline.py), so AUTO takes it only when the per-tile grid would fill < 40 % of the SMs.
     // VCB_SP_ATTN_PERSIST=0 / 1 forces it off / on.
     static const int sp_persist_env = [] { const char* e = getenv("VCB_SP_ATTN_PERSIST"); return e ? (atoi(e) ? 1 : 0) : -1; }();
     const bool sp_persist = out_peers && (sp_persist_env >= 0 ? sp_persist_env == 1 : n_units * 10 < (long long)num_sms() * 4);
     const bool persist_ok = !seqlens && (!out_peers || sp_persist) && num_sms() <= 160 && n_units / pgrid + 4 <= kAttn4MaxSegs;
     if (schedule == VCB_ATTN_SCHED_PERSISTENT && !persist_ok)
         return set_error("attention: the persistent schedule takes unpadded batches (seqlens == NULL), no sequence-parallel routing");
+    AttnSkParams skp{nullptr, nullptr, 0, 0, nullptr};
+    dim3 grid((unsigned)n_qt, heads, B);
     if (persist_ok && (schedule == VCB_ATTN_SCHED_PERSISTENT || (schedule == VCB_ATTN_SCHED_AUTO && (attn_persist_mode() != 0 || sp_persist)))) {
-        const int grid = pgrid;
+        grid = dim3(pgrid);
         prof.set_info(3, (fixed ? 1 : 0) | 2);
         AttnScratch* sc = attn_scratch((cudaStream_t)stream);
         if (!sc) return set_error("attention: workspace allocation failed");
         static const int no_split = [] { const char* e = getenv("VCB_ATTN4_NOSPLIT"); return (e && atoi(e)) ? 1 : 0; }();
-        AttnSkParams skp{sc->ws, sc->flags, ++sc->epoch, no_split, sc->timeline};
+        skp = AttnSkParams{sc->ws, sc->flags, ++sc->epoch, no_split, sc->timeline};
         if (sc->timeline) cudaMemsetAsync(sc->timeline, 0, 160 * (kAttn4MaxSegs + 2) * sizeof(unsigned long long), (cudaStream_t)stream);
-        sc->last_grid = grid;
+        sc->last_grid = pgrid;
         g_last_attn_scratch = sc;
-        cudaError_t e = fixed ? launch_pdl(attn_fwd4_tcgen05_kernel<true>, dim3(grid), dim3(kAttn3Threads), (size_t)kAttn4SmemBytes, (cudaStream_t)stream, 1, tm, p, skp)
-                              : launch_pdl(attn_fwd4_tcgen05_kernel<false>, dim3(grid), dim3(kAttn3Threads), (size_t)kAttn4SmemBytes, (cudaStream_t)stream, 1, tm, p, skp);
-        if (e != cudaSuccess) return set_error("attention (persistent) launch: %s", cudaGetErrorString(e));
-        count_launch();
-        return 0;
     }
-    static const bool sp_direct = [] { const char* e = getenv("VCB_SP_ATTN_DIRECT"); return e && atoi(e); }();
-    if (out_peers && !sp_direct) {
-        // staged TMA tile stores into the row owners' buffers (NVLink for remote owners)
-        AttnSpMapsT<true> spm{};
-        for (int r = 0; r < world; ++r)
-            if (int rc = make_tmap_2d(&spm.m[r], out_peers[r], (uint64_t)ldo, (uint64_t)rows_per_rank, (uint64_t)ldo, 64, 32)) return rc;
-        dim3 grid((L + 2 * kAttnTile - 1) / (2 * kAttnTile), heads, B);
-        cudaError_t e = fixed ? launch_pdl(attn_fwd3_tcgen05_kernel<true, 2, true>, grid, dim3(kAttn3Threads), (size_t)kAttn3SmemBytes, (cudaStream_t)stream, 1, tm, p, spm)
-                              : launch_pdl(attn_fwd3_tcgen05_kernel<true, 2>, grid, dim3(kAttn3Threads), (size_t)kAttn3SmemBytes, (cudaStream_t)stream, 1, tm, p, spm);
-        if (e != cudaSuccess) return set_error("attention (sp) launch: %s", cudaGetErrorString(e));
-        count_launch();
-        return 0;
-    }
-    {
-        dim3 grid((L + 2 * kAttnTile - 1) / (2 * kAttnTile), heads, B);
-        cudaError_t e = fixed ? launch_pdl(attn_fwd3_tcgen05_kernel<false, 2, true>, grid, dim3(kAttn3Threads), (size_t)kAttn3SmemBytes, (cudaStream_t)stream, 1, tm, p, AttnSpMapsT<false>{})
-                              : launch_pdl(attn_fwd3_tcgen05_kernel<false, 2>, grid, dim3(kAttn3Threads), (size_t)kAttn3SmemBytes, (cudaStream_t)stream, 1, tm, p, AttnSpMapsT<false>{});
-        if (e != cudaSuccess) return set_error("attention launch: %s", cudaGetErrorString(e));
-        count_launch();
-        return 0;
-    }
+    cudaError_t e = fixed ? launch_pdl(attn_fwd_wgmma_kernel<true>, grid, dim3(kAttnThreads), (size_t)kAttnSmemBytes, (cudaStream_t)stream, 1, tm, p, skp)
+                          : launch_pdl(attn_fwd_wgmma_kernel<false>, grid, dim3(kAttnThreads), (size_t)kAttnSmemBytes, (cudaStream_t)stream, 1, tm, p, skp);
+    if (e != cudaSuccess) return set_error("attention launch: %s", cudaGetErrorString(e));
+    count_launch();
+    return 0;
 }
 }  // namespace
 
@@ -845,13 +798,13 @@ extern "C" int vcb_copy_cols(const void* src, int64_t lds, void* dst, int64_t ld
 // probe
 // ------------------------------------------------------------------------------------------------
 extern "C" int vcb_debug_umma_probe(const void* a, const void* b, float* out, int32_t ksteps, int32_t b_mn_major,
-                                    int32_t a_from_tmem, uint32_t b_lbo, uint32_t b_sbo, uint32_t b_kstep_bytes,
+                                    int32_t a_from_regs, uint32_t b_lbo, uint32_t b_sbo, uint32_t b_kstep_bytes,
                                     void* stream) {
     if (!a || !b || !out || (ksteps != 4 && ksteps != 8)) return set_error("probe: ksteps must be 4 or 8");
     if (int rc = ensure_device()) return rc;
     const int K = 16 * ksteps;
     static std::once_flag once;
-    std::call_once(once, [&] { cudaFuncSetAttribute(umma_probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 67 * 1024); });
+    std::call_once(once, [&] { cudaFuncSetAttribute(wgmma_probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 67 * 1024); });
     CUtensorMap ta, tb;
     if (int rc = make_tmap_2d(&ta, a, (uint64_t)K, 128, (uint64_t)K, 64, 128)) return rc;
     if (b_mn_major) {
@@ -859,8 +812,8 @@ extern "C" int vcb_debug_umma_probe(const void* a, const void* b, float* out, in
     } else {
         if (int rc = make_tmap_2d(&tb, b, (uint64_t)K, 128, (uint64_t)K, 64, 128)) return rc;
     }
-    ProbeParams p{(const __nv_bfloat16*)a, out, ksteps, b_mn_major, a_from_tmem, b_lbo, b_sbo, b_kstep_bytes};
-    umma_probe_kernel<<<1, 192, 67 * 1024, (cudaStream_t)stream>>>(ta, tb, p);
+    ProbeParams p{(const __nv_bfloat16*)a, out, ksteps, b_mn_major, a_from_regs, b_lbo, b_sbo, b_kstep_bytes};
+    wgmma_probe_kernel<<<1, 288, 67 * 1024, (cudaStream_t)stream>>>(ta, tb, p);
     return check_launch("umma_probe");
 }
 

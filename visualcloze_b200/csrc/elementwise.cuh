@@ -208,7 +208,7 @@ ln_modulate2_kernel(const LnProblem p0, const LnProblem p1, long long ldx, long 
 }
 
 // Statistics-from-the-producer variant: the GATE_RES epilogue of the GEMM that wrote the residual stream also left, per row, one
-// (sum, sum of squares) pair per 64 columns (gemm_sm100.cuh, row_stats).  The LayerNorm then needs no pass over the row for its
+// (sum, sum of squares) pair per 64 columns (gemm_sm90.cuh, row_stats).  The LayerNorm then needs no pass over the row for its
 // statistics: a warp adds the row's n_slots pairs in a fixed order (deterministic), and streams the row ONCE.
 struct LnStatsProblem {
     const __nv_bfloat16* x; __nv_bfloat16* y;

@@ -136,8 +136,8 @@ inline DeviceInfo& device_info() {
         cudaDeviceGetAttribute(&info.sms, cudaDevAttrMultiProcessorCount, dev);
         cudaDeviceGetAttribute(&info.cc_major, cudaDevAttrComputeCapabilityMajor, dev);
         cudaDeviceGetAttribute(&info.cc_minor, cudaDevAttrComputeCapabilityMinor, dev);
-        if (info.cc_major != 10) {
-            snprintf(info.err, sizeof(info.err), "device is sm_%d%d; libvcb200 is built for sm_100a only", info.cc_major, info.cc_minor);
+        if (info.cc_major != 9) {
+            snprintf(info.err, sizeof(info.err), "device is sm_%d%d; libvcb200 is built for sm_90a only", info.cc_major, info.cc_minor);
             return;
         }
         info.ok = 1;

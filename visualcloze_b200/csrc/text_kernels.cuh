@@ -1,6 +1,6 @@
 // text_kernels.cuh -- the non-GEMM pieces of the two text encoders behind models/modules/conditioner.py:5-37 (SURVEY.md 8f-4):
 // T5 v1.1 encoder (HF T5EncoderModel: T5LayerNorm, relative-position-bias attention, gated GELU) and the CLIP-L text model
-// (nn.LayerNorm, causal attention, quick-GELU).  Everything with a matrix in it goes through gemm_sm100.cuh; what is left is
+// (nn.LayerNorm, causal attention, quick-GELU).  Everything with a matrix in it goes through gemm_sm90.cuh; what is left is
 // HBM-bound row work and a small attention (head_dim 64, at most 512 keys, 4.3 GFLOP per T5 layer) that runs on the CUDA cores.
 // Rounding points follow the bf16 HF modules the reference loads (torch_dtype=torch.bfloat16, models/util.py:425-431).
 #pragma once

@@ -1,7 +1,7 @@
 // vae_kernels.cuh -- HBM-bound kernels of the VAE decoder (models/modules/autoencoder.py): GroupNorm(32)+swish,
 // nearest 2x upsampling, row softmax of the mid-block attention, latent-token / image layout conversions.
 // Activations are NHWC bf16 so that a pixel's channels are one contiguous, 16-byte-vectorisable run and the 3x3
-// convolutions are implicit GEMMs (gemm_sm100.cuh, A_CONV3X3).
+// convolutions are implicit GEMMs (gemm_sm90.cuh, A_CONV3X3).
 #pragma once
 #include "vcb_common.cuh"
 

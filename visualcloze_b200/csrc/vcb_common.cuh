@@ -1,5 +1,5 @@
-// vcb_common.cuh -- sm_100a PTX wrappers shared by the vcb200 kernels (mbarrier, TMA, tcgen05/TMEM).
-// Hand-written inline PTX; bit layouts follow the PTX ISA "tcgen05" matrix/instruction descriptors.
+// vcb_common.cuh -- sm_90a PTX wrappers shared by the vcb200 kernels (mbarrier, TMA, wgmma operand descriptors).
+// Hand-written inline PTX; bit layouts follow the PTX ISA "wgmma" matrix descriptor.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -106,247 +106,74 @@ VCB_DEVICE void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" 
 VCB_DEVICE void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }   // smem reusable
 VCB_DEVICE void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }         // writes done
 
-// kPeer: 2-CTA mode -- the transaction bytes are credited to the leader CTA's barrier.
-template <bool kPeer>
-VCB_DEVICE void tma_load_2d(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1, uint64_t hint) {
-    uint32_t b = smem_u32(bar);
-    if constexpr (kPeer) {
-        b &= 0xFEFFFFFFu;
+// kMulticast: the tile lands at the same shared-memory offset in every CTA of `mask` (a 2-CTA cluster sharing one B tile) and
+// completes the transaction bytes on the barrier at the same offset in each of them.
+template <bool kMulticast = false>
+VCB_DEVICE void tma_load_2d(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1, uint64_t hint, uint16_t mask = 0) {
+    if constexpr (kMulticast) {
         asm volatile(
-            "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-            " [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(smem_u32(dst)),
-            "l"(reinterpret_cast<uint64_t>(m)), "r"(b), "r"(c0), "r"(c1), "l"(hint)
+            "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster.L2::cache_hint"
+            " [%0], [%1, {%3, %4}], [%2], %5, %6;" ::"r"(smem_u32(dst)),
+            "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(mask), "l"(hint)
             : "memory");
     } else {
         asm volatile(
             "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
             " [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(smem_u32(dst)),
-            "l"(reinterpret_cast<uint64_t>(m)), "r"(b), "r"(c0), "r"(c1), "l"(hint)
+            "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "l"(hint)
             : "memory");
     }
 }
-template <bool kPeer>
 VCB_DEVICE void tma_load_3d(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1, int c2, uint64_t hint) {
-    uint32_t b = smem_u32(bar);
-    if constexpr (kPeer) {
-        b &= 0xFEFFFFFFu;
-        asm volatile(
-            "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-            " [%0], [%1, {%3, %4, %5}], [%2], %6;" ::"r"(smem_u32(dst)),
-            "l"(reinterpret_cast<uint64_t>(m)), "r"(b), "r"(c0), "r"(c1), "r"(c2), "l"(hint)
-            : "memory");
-    } else {
-        asm volatile(
-            "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-            " [%0], [%1, {%3, %4, %5}], [%2], %6;" ::"r"(smem_u32(dst)),
-            "l"(reinterpret_cast<uint64_t>(m)), "r"(b), "r"(c0), "r"(c1), "r"(c2), "l"(hint)
-            : "memory");
-    }
+    asm volatile(
+        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
+        " [%0], [%1, {%3, %4, %5}], [%2], %6;" ::"r"(smem_u32(dst)),
+        "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "l"(hint)
+        : "memory");
 }
-template <bool kPeer>
-VCB_DEVICE void tma_load_4d(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1, int c2, int c3,
-                            uint64_t hint) {
-    uint32_t b = smem_u32(bar);
-    if constexpr (kPeer) {
-        b &= 0xFEFFFFFFu;
-        asm volatile(
-            "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-            " [%0], [%1, {%3, %4, %5, %6}], [%2], %7;" ::"r"(smem_u32(dst)),
-            "l"(reinterpret_cast<uint64_t>(m)), "r"(b), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "l"(hint)
-            : "memory");
-    } else {
-        asm volatile(
-            "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-            " [%0], [%1, {%3, %4, %5, %6}], [%2], %7;" ::"r"(smem_u32(dst)),
-            "l"(reinterpret_cast<uint64_t>(m)), "r"(b), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "l"(hint)
-            : "memory");
-    }
+VCB_DEVICE void tma_load_4d(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1, int c2, int c3, uint64_t hint) {
+    asm volatile(
+        "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
+        " [%0], [%1, {%3, %4, %5, %6}], [%2], %7;" ::"r"(smem_u32(dst)),
+        "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "l"(hint)
+        : "memory");
 }
 
 // ------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, fences, commit, MMA, ld/st
+// wgmma operands (the instruction wrappers are in wgmma_sm90.cuh)
 // ------------------------------------------------------------------------------------------
-template <int kCtaGroup>
-VCB_DEVICE void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-    if constexpr (kCtaGroup == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-                     "r"(ncols)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    } else {
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-                     "r"(ncols)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-}
-template <int kCtaGroup>
-VCB_DEVICE void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    if constexpr (kCtaGroup == 1)
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-    else
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-VCB_DEVICE void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-VCB_DEVICE void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-VCB_DEVICE void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-VCB_DEVICE void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// tcgen05.commit: arrive on `bar` once all previously issued MMAs of this thread have completed.
-// kCtaGroup == 2: multicast the arrive to the same barrier offset in both CTAs of the pair.
-template <int kCtaGroup>
-VCB_DEVICE void umma_commit(uint64_t* bar) {
-    if constexpr (kCtaGroup == 1) {
-        asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                     : "memory");
-    } else {
-        asm volatile(
-            "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                smem_u32(bar)),
-            "h"((uint16_t)3)
-            : "memory");
-    }
-}
-
-// Instruction descriptor, kind::f16, bf16 x bf16 -> fp32 (PTX ISA "Instruction descriptor").
-//   [4,6) D format (1 = f32)  [7,10) A format (1 = bf16)  [10,13) B format (1 = bf16)
-//   [15] A major (0 = K)  [16] B major (0 = K, 1 = MN)  [17,23) N >> 3  [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, int a_mn_major, int b_mn_major) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) |
-           ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-// kind::f8f6f4 with both operands e4m3 (format code 0 in [7,10) and [10,13)), fp32 accumulate, K-major x K-major
-__host__ __device__ constexpr uint32_t make_idesc_e4m3(int M, int N) {
-    return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-// Shared-memory matrix descriptor (PTX ISA "Matrix descriptor", sm_100 version field = 1).
+// Shared-memory matrix descriptor (PTX ISA "Matrix descriptor" of wgmma):
 //   [0,14) start address >> 4   [16,30) leading-dim byte offset >> 4   [32,46) stride-dim byte offset >> 4
-//   [46,48) version = 1         [61,64) swizzle: 0 none, 2 = 128B, 4 = 64B, 6 = 32B
-VCB_DEVICE uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout_type) {
+//   [62,64) swizzle: 0 none, 1 = 128B, 2 = 64B, 3 = 32B
+// K-major 128B-swizzled operand: rows of 128 bytes, SBO = 1024 (8 rows), LBO unused; a 16-element k step is +32 bytes.
+// MN-major 128B-swizzled operand: LBO = distance between 64-element column blocks, SBO = 1024 (8 k rows).
+VCB_DEVICE uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)(layout_type & 7u) << 61;
+    d |= (uint64_t)1 << 62;                      // 128-byte swizzle
     return d;
 }
-constexpr uint32_t kSwizzle128B = 2;
 
-// D[tmem] (+)= A[smem] * B[smem]; kFp8: kind::f8f6f4 (8-bit operands, K = 32 per instruction) instead of kind::f16
-template <int kCtaGroup, bool kFp8 = false>
-VCB_DEVICE void umma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    if constexpr (kFp8) {
-        if constexpr (kCtaGroup == 1) {
-            asm volatile(
-                "{\n\t.reg .pred p;\n\t"
-                "setp.ne.b32 p, %4, 0;\n\t"
-                "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-                "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-                : "memory");
-        } else {
-            asm volatile(
-                "{\n\t.reg .pred p;\n\t"
-                "setp.ne.b32 p, %4, 0;\n\t"
-                "tcgen05.mma.cta_group::2.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-                "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-                : "memory");
-        }
-    } else if constexpr (kCtaGroup == 1) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "setp.ne.b32 p, %4, 0;\n\t"
-            "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-            "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-            : "memory");
-    } else {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "setp.ne.b32 p, %4, 0;\n\t"
-            "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-            "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-            : "memory");
-    }
-}
-// D[tmem] (+)= A[tmem] * B[smem]
-VCB_DEVICE void umma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-        "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
+// warp-specialised kernels hand the producer warpgroup's registers to the consumers (counts are multiples of 8)
+template <int kRegs>
+VCB_DEVICE void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegs)); }
+template <int kRegs>
+VCB_DEVICE void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegs)); }
 
-// TMEM -> registers, 32 lanes x 32-bit, N consecutive columns per thread (thread t <-> lane base+t)
-VCB_DEVICE void tmem_ld_x32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-}
-VCB_DEVICE void tmem_ld_x16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-}
-VCB_DEVICE void tmem_st_x32(uint32_t taddr, const uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-        "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-        "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-        "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-        "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-        : "memory");
-}
-VCB_DEVICE void tmem_st_x16(uint32_t taddr, const uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-        "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-        "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-        : "memory");
-}
-VCB_DEVICE void tmem_st_x8(uint32_t taddr, const uint32_t (&r)[8]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(r[0]), "r"(r[1]),
-                 "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-                 : "memory");
-}
-
-// fast math used by the softmax inner loop: single-instruction ex2, packed fp32x2 FMA / ADD (FFMA2 / FADD2 on sm_100)
 VCB_DEVICE float ex2_approx(float x) {
     float y;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
 }
-VCB_DEVICE uint64_t pack_f32x2(float lo, float hi) {
-    uint64_t r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-    return r;
+
+VCB_DEVICE int ld_acquire_gpu(const int* p) {
+    int v;
+    asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
 }
-VCB_DEVICE void unpack_f32x2(uint64_t r, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(r)); }
-VCB_DEVICE uint64_t fma_f32x2(uint64_t a, uint64_t b, uint64_t c) {
-    uint64_t r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-    return r;
-}
-VCB_DEVICE uint64_t add_f32x2(uint64_t a, uint64_t b) {
-    uint64_t r;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
-}
+VCB_DEVICE void st_release_gpu(int* p, int v) { asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
 
 // Programmatic dependent launch: let the next kernel's CTAs start (and run their prologue) while this grid drains;
 // `pdl_wait` blocks until the preceding grid has completed and its writes are visible.

@@ -216,7 +216,7 @@ class FluxEngine:
             n_img = im.sum(dim=-1, dtype=torch.int32)
             prefix = torch.arange(Li, device=dev)[None, :] < n_img[:, None]
             if not bool(tm.all() & (im == prefix).all()):
-                raise ValueError("unsupported attention mask: the sm_100a attention kernel takes a fully valid txt_mask and a "
+                raise ValueError("unsupported attention mask: the sm_90a attention kernel takes a fully valid txt_mask and a "
                                  "right-padded (prefix) img_mask -- the layout prepare_modified produces (models/sampling.py:82-98)")
             if img_mask is not None:
                 seqlens = (n_img + Lt).contiguous()

@@ -13,7 +13,7 @@ Mirror of ``models/model.py`` (``FluxParams`` :18-32, ``Flux`` :35-151, ``FluxLo
     (``W' = W + s * B A``, ``b' = b + s * b_B``), re-packed when the scale or a parameter changes.
 
 The module holds parameters only; all arithmetic happens in the CUDA library (``engine.py``).  There is no
-PyTorch fallback: calling ``forward`` without a B200 raises.
+PyTorch fallback: calling ``forward`` without an H100 raises.
 """
 from __future__ import annotations
 
@@ -112,7 +112,7 @@ class Flux(nn.Module):
         if sum(params.axes_dim) != pe_dim:
             raise ValueError(f"Got {params.axes_dim} but expected positional dim {pe_dim}")
         if pe_dim != 128:
-            raise ValueError("the sm_100a kernels are specialised for head_dim 128")
+            raise ValueError("the sm_90a kernels are specialised for head_dim 128")
         self.hidden_size = params.hidden_size
         self.num_heads = params.num_heads
         self.lora_rank = 0

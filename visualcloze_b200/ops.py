@@ -322,9 +322,9 @@ def copy_cols(src, dst, col0: int) -> torch.Tensor:
     return dst
 
 
-def umma_probe(a, b, ksteps: int, b_mn_major: bool, a_from_tmem: bool, b_lbo: int = 0, b_sbo: int = 0,
+def umma_probe(a, b, ksteps: int, b_mn_major: bool, a_from_regs: bool, b_lbo: int = 0, b_sbo: int = 0,
                b_kstep_bytes: int = 0) -> torch.Tensor:
     out = torch.empty(128, 128, dtype=torch.float32, device=a.device)
     check(_lib.lib().vcb_debug_umma_probe(a.data_ptr(), b.data_ptr(), out.data_ptr(), ksteps, int(b_mn_major),
-                                          int(a_from_tmem), b_lbo, b_sbo, b_kstep_bytes, _stream()), "vcb_debug_umma_probe")
+                                          int(a_from_regs), b_lbo, b_sbo, b_kstep_bytes, _stream()), "vcb_debug_umma_probe")
     return out

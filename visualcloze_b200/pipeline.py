@@ -1,4 +1,4 @@
-"""``VisualClozeModel`` -- the reference's inference entry point on the B200-native hot path.
+"""``VisualClozeModel`` -- the reference's inference entry point on the H100-native hot path.
 
 Mirror of ``visualcloze.py:78-467``: same constructor arguments, ``set_grid_size``, ``process_images`` and ``upsampling``
 signatures and return types (list of PIL images / PIL image), same image preparation, mask/cond packing, seeding,
@@ -120,7 +120,7 @@ class VisualClozeModel:
         ``model`` / ``ae_decoder`` / ``ae_encoder`` objects are used as they are.  Nothing is ever run on never-loaded
         parameters: the engines refuse to pack them."""
         if precision != "bf16":
-            raise NotImplementedError("the sm_100a kernels implement the reference's default bf16 path only")
+            raise NotImplementedError("the sm_90a kernels implement the reference's default bf16 path only")
         if model_name != "flux-dev-fill-lora":
             raise NotImplementedError("VisualCloze uses the flux-dev-fill-lora geometry (models/util.py:132-165)")
         self.atol, self.rtol, self.solver = atol, rtol, solver
