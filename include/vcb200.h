@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define VCB_ABI_VERSION 6
+#define VCB_ABI_VERSION 7
 #define VCB_SP_MAX 8          /* ranks of one sequence-parallel group (one NVSwitch domain) */
 
 /* ---- library ------------------------------------------------------------------------------ */
@@ -46,7 +46,8 @@ int         vcb_profile_end_ex(double* ms, long long* launches, int32_t ncat, vc
 
 /* ---- fused-epilogue GEMM:  D = epilogue(A[M,K] * W[N,K]^T)   (bf16 x bf16 -> fp32 -> bf16) --------------
  * Replaces every nn.Linear on the path (models/modules/layers.py:165,172,190-195,235,244; model.py:101,108;
- * lora.py:92-98 with merged weights) together with the elementwise ops that follow it in the reference. */
+ * lora.py:92-98 with merged weights, or unmerged through the LoRA k-tail below) together with the elementwise ops that
+ * follow it in the reference. */
 enum vcb_epilogue {
     VCB_EPI_BIAS = 0,      /* out = bf16(acc + bias) */
     VCB_EPI_BIAS_GELU = 1, /* out = bf16(gelu_tanh(bf16(acc + bias)))                    layers.py:143,154 */
@@ -100,6 +101,17 @@ typedef struct vcb_gemm_args {
     int32_t operand_dtype;           /* VCB_DTYPE_BF16 (0) or VCB_DTYPE_E4M3 (1) */
     const float* a_scale;
     const float* w_scale;
+    /* Unmerged LoRA k-tail (bf16 operands only; lora_rank 0 = none): out = epilogue(A W^T + T lora_b^T), one fp32 accumulator,
+       i.e. [A | T] [W | lora_b]^T.  T [M, lora_rank] bf16 is addressed like A: row i of sample b at
+       lora_t + b * lora_t_batch_stride + i * ld_lora_t (batch stride 0 = rows_per_batch * ld_lora_t).  lora_b [N, lora_rank] bf16
+       (row stride lora_rank, lora.py's lora_B.weight).  lora_rank % 8 == 0 (the last partial k-block is zero-filled); both problems
+       of a grouped launch need the same rank. */
+    const void* lora_t; int64_t ld_lora_t;
+    int64_t lora_t_batch_stride;
+    const void* lora_b;
+    int32_t lora_rank;
+    /* output scale: the epilogue sees alpha * acc in place of acc (0 = 1).  The LoRA down-projection T = bf16(s * X lora_a^T). */
+    float alpha;
 } vcb_gemm_args;
 #define VCB_DTYPE_BF16 0
 #define VCB_DTYPE_E4M3 1
@@ -239,12 +251,19 @@ int vcb_copy_cols(const void* src, int64_t lds, void* dst, int64_t ldd, int32_t 
 
 
 /* ---- FLUX-DiT engine: the whole Flux.forward (models/model.py:85-124) and the Euler loop around it -----------
- * Weights are the reference's tensors with LoRA merged (W' = W + s*B*A, b' = b + s*b_B; lora.py:92-98), bf16
- * weights [out, in], fp32 biases.  The engine keeps pointers only; the caller owns weights and workspace. */
+ * Weights are the reference's tensors in one of two forms, chosen per Linear (lora.py:92-98): LoRA merged (rank 0:
+ * w = W + s*B*A) or unmerged (rank > 0: w = W, lora_a = A [rank, in], lora_b = B [out, rank], lora_scale = s; every call then
+ * runs the down-projection T = bf16(s * x A^T) and the main GEMM with the LoRA k-tail, vcb_gemm_args.lora_*).  Either way
+ * b = b + s*b_B; bf16 weights [out, in], fp32 biases.  The engine keeps pointers only; the caller owns weights and workspace. */
 /* w8 / w8_scale (optional): the same merged weight quantised to e4m3 with one fp32 scale per output channel (w ~= w8 * scale),
  * used by the opt-in fp8 projections (vcb_flux_set_fp8): level 1 needs it on the LayerNorm-fed Linears (qkv, mlp.0, linear1), level 2
  * also on attn.proj, mlp.2 and linear2; NULL = bf16 only. */
-typedef struct vcb_linear_w { const void* w; const float* b; const void* w8; const float* w8_scale; } vcb_linear_w;
+/* lora_a / lora_b / rank / lora_scale: the unmerged LoRA form (rank % 8 == 0; rank 0 or lora_scale 0 = no update); bf16 only, so
+ * an engine holding an unmerged Linear refuses vcb_flux_set_fp8 and vcb_flux_sp_attach. */
+typedef struct vcb_linear_w {
+    const void* w; const float* b; const void* w8; const float* w8_scale;
+    const void* lora_a; const void* lora_b; int32_t rank; float lora_scale;
+} vcb_linear_w;
 
 typedef struct vcb_stream_w {           /* one stream of a DoubleStreamBlock (layers.py:129-156) */
     vcb_linear_w mod, qkv, proj, mlp0, mlp2;
@@ -289,7 +308,8 @@ int  vcb_flux_use_score_bounds(vcb_flux* f, int32_t enable);
 #define VCB_FP8_LN_FED 1
 #define VCB_FP8_ALL_LINEARS 2
 int  vcb_flux_set_fp8(vcb_flux* f, int32_t level);
-/* bytes of device workspace for B samples of Li image + Lt text tokens and n_evals model evaluations */
+/* bytes of device workspace for B samples of Li image + Lt text tokens and n_evals model evaluations (with unmerged LoRA
+ * Linears: + the down-projection buffer T [max(B * (Li + Lt), n_evals * B), largest rank] bf16) */
 int64_t vcb_flux_workspace_bytes(const vcb_flux* f, int32_t B, int32_t Li, int32_t Lt, int32_t n_evals);
 /* Step-invariant work, once per image (SURVEY.md 2.2: txt_in, RoPE table, and the AdaLN modulation vectors of
  * all n_evals steps as one batched GEMM per block).  t_scaled: [n_evals * B] fp32 = 1000 * flux_time (row e*B+b);

@@ -6,7 +6,7 @@ import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libvcb200.so")
-ABI_VERSION = 6
+ABI_VERSION = 7
 SP_MAX = 8
 
 _lib = None
@@ -37,6 +37,8 @@ class GemmArgs(C.Structure):
         ("sp_world", C.c_int32), ("sp_row_offset", C.c_int32), ("sp_out", C.c_void_p * SP_MAX),
         ("row_stats", C.c_void_p),
         ("operand_dtype", C.c_int32), ("a_scale", C.c_void_p), ("w_scale", C.c_void_p),
+        ("lora_t", C.c_void_p), ("ld_lora_t", C.c_int64), ("lora_t_batch_stride", C.c_int64), ("lora_b", C.c_void_p),
+        ("lora_rank", C.c_int32), ("alpha", C.c_float),
     ]
 
 
@@ -78,7 +80,9 @@ _SIGNATURES = {
 }
 
 class LinearW(C.Structure):
-    _fields_ = [("w", C.c_void_p), ("b", C.c_void_p), ("w8", C.c_void_p), ("w8_scale", C.c_void_p)]
+    """struct vcb_linear_w (include/vcb200.h): rank 0 = merged weight, rank > 0 = unmerged LoRA (w, lora_a, lora_b, lora_scale)."""
+    _fields_ = [("w", C.c_void_p), ("b", C.c_void_p), ("w8", C.c_void_p), ("w8_scale", C.c_void_p),
+                ("lora_a", C.c_void_p), ("lora_b", C.c_void_p), ("rank", C.c_int32), ("lora_scale", C.c_float)]
 
 
 class StreamW(C.Structure):

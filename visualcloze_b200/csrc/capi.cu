@@ -22,7 +22,7 @@ using namespace vcb;
 // ------------------------------------------------------------------------------------------------
 namespace {
 
-struct Problem { CUtensorMap ta, tb; GemmParams p; };
+struct Problem { CUtensorMap ta, tb, tt, tl; GemmParams p; };      // tt / tl: LoRA k-tail maps (T, lora_b); copies of ta / tb without one
 
 // stream-K scratch: one slot of 128 x 256 fp32 per CTA and one flag per CTA, per stream (launches on one stream are
 // ordered, so a single scratch per stream is enough); allocated on first use (call once before CUDA-graph capture)
@@ -82,14 +82,15 @@ int launch_gemm_inst(const Problem& g0, const Problem& g1, float rate, cudaStrea
     int clusters = num_sms() / CG;
     // stream-K tail: the tiles of the partial last wave are cut along K into one equal range per CTA (pair)
     StreamKParams skp{nullptr, nullptr, 0, 0};
-    const bool sk = streamk_wanted(tiles, clusters, tile_time_us(BN, p.K, rate) * (FP8 ? 0.5f : 1.0f));
+    const bool sk = streamk_wanted(tiles, clusters, tile_time_us(BN, p.K + p.lora_rank, rate) * (FP8 ? 0.5f : 1.0f));
     if (tiles < clusters && !sk) clusters = tiles;
     if (sk) {
         SkScratch* sc = sk_scratch(st);
         if (!sc) return set_error("gemm: stream-K scratch allocation failed");
         skp.ws = sc->ws; skp.flags = sc->flags; skp.epoch = ++sc->epoch; skp.enabled = 1;
     }
-    cudaError_t e = launch_pdl(kern, dim3(clusters * CG), dim3(kGemmThreads), (size_t)kSmem, st, CG, ta, tb, p, g1.ta, g1.tb, g1.p, skp);
+    cudaError_t e = launch_pdl(kern, dim3(clusters * CG), dim3(kGemmThreads), (size_t)kSmem, st, CG, ta, tb, p, g1.ta, g1.tb, g1.p, skp,
+                               g0.tt, g0.tl, g1.tt, g1.tl);
     if (e != cudaSuccess) return set_error("gemm launch (BN=%d CG=%d EPI=%d): %s", BN, CG, EPI, cudaGetErrorString(e));
     count_launch();
     return 0;
@@ -218,6 +219,12 @@ int check_gemm_args(const vcb_gemm_args* a) {
         if (reinterpret_cast<uintptr_t>(a->w_scale) & 15) return set_error("gemm (fp8): w_scale must be 16-byte aligned (read as float4)");
         if (a->block_n && a->block_n != 128 && a->block_n != 256) return set_error("gemm (fp8): block_n must be 128 or 256");
     }
+    if (a->lora_rank < 0 || a->lora_rank % 8) return set_error("gemm: lora_rank must be a non-negative multiple of 8 (16-byte rows of T and lora_b)");
+    if (a->lora_rank > 0) {
+        if (!a->lora_t || !a->lora_b) return set_error("gemm: a LoRA k-tail (lora_rank > 0) needs lora_t and lora_b");
+        if (a->operand_dtype == VCB_DTYPE_E4M3) return set_error("gemm (fp8): the LoRA k-tail takes bf16 operands");
+        if (a->ld_lora_t % 8 || a->lora_t_batch_stride % 8) return set_error("gemm: ld_lora_t and lora_t_batch_stride must be multiples of 8");
+    }
     return 0;
 }
 
@@ -237,6 +244,7 @@ int build_problem(const vcb_gemm_args* a, int bn, int cg, Problem* out) {
     p.rope = (const float2*)a->rope; p.rope_rows = a->rope_rows;
     p.out2 = (__nv_bfloat16*)a->out2; p.ldo2 = a->ldo2; p.out2_col_offset = a->out2_col_offset;
     p.sp_world = a->sp_world > 1 ? a->sp_world : 0; p.sp_row_offset = a->sp_row_offset;
+    p.lora_rank = a->lora_rank; p.alpha = a->alpha;
     const bool fp8 = a->operand_dtype == VCB_DTYPE_E4M3;
     const int eb = fp8 ? 1 : 2;                    // operand bytes per element; a k-block is 128 bytes of K either way
     p.a_scale = fp8 ? a->a_scale : nullptr; p.w_scale = fp8 ? a->w_scale : nullptr;
@@ -244,6 +252,13 @@ int build_problem(const vcb_gemm_args* a, int bn, int cg, Problem* out) {
     if (int rc = make_tmap_3d(&out->ta, a->A, (uint64_t)a->K, (uint64_t)a->rows_per_batch, (uint64_t)batch, (uint64_t)a->lda,
                               (uint64_t)a_bstride, 128 / eb, 128, eb)) return rc;
     if (int rc = make_tmap_2d(&out->tb, a->W, (uint64_t)a->K, (uint64_t)a->N, (uint64_t)a->ldw, 128 / eb, (uint32_t)(bn / cg), eb)) return rc;
+    out->tt = out->ta; out->tl = out->tb;
+    if (a->lora_rank > 0) {
+        const int64_t t_bstride = a->lora_t_batch_stride ? a->lora_t_batch_stride : (int64_t)a->rows_per_batch * a->ld_lora_t;
+        if (int rc = make_tmap_3d(&out->tt, a->lora_t, (uint64_t)a->lora_rank, (uint64_t)a->rows_per_batch, (uint64_t)batch,
+                                  (uint64_t)a->ld_lora_t, (uint64_t)t_bstride, 64, 128)) return rc;
+        if (int rc = make_tmap_2d(&out->tl, a->lora_b, (uint64_t)a->lora_rank, (uint64_t)a->N, (uint64_t)a->lora_rank, 64, (uint32_t)(bn / cg))) return rc;
+    }
     return 0;
 }
 
@@ -252,8 +267,8 @@ int gemm_dispatch(const vcb_gemm_args* a, const vcb_gemm_args* a1, void* stream)
     if (a1) {
         if (int rc = check_gemm_args(a1)) return rc;
         if (a1->N != a->N || a1->K != a->K || a1->epilogue != a->epilogue || (a1->sp_world > 1) != (a->sp_world > 1) ||
-            a1->operand_dtype != a->operand_dtype)
-            return set_error("gemm (grouped): both problems need the same N, K, epilogue, operand dtype and sequence-parallel mode");
+            a1->operand_dtype != a->operand_dtype || a1->lora_rank != a->lora_rank)
+            return set_error("gemm (grouped): both problems need the same N, K, LoRA rank, epilogue, operand dtype and sequence-parallel mode");
     }
     if (int rc = ensure_device()) return rc;
     const bool head = a->epilogue == VCB_EPI_QKV || a->epilogue == VCB_EPI_LINEAR1;
@@ -263,7 +278,7 @@ int gemm_dispatch(const vcb_gemm_args* a, const vcb_gemm_args* a1, void* stream)
     float rate;
     const bool fp8 = a->operand_dtype == VCB_DTYPE_E4M3;
     const bool stats = a->row_stats || (a1 && a1->row_stats);      // 64-column statistics slots: tiles of 128 or 256 columns
-    pick_tile(batch, a->rows_per_batch + (a1 ? a1->M / batch : 0), a->N, a->K, head || fp8 || stats, a->cta_group ? a->cta_group : forced_cta_group(),
+    pick_tile(batch, a->rows_per_batch + (a1 ? a1->M / batch : 0), a->N, a->K + a->lora_rank, head || fp8 || stats, a->cta_group ? a->cta_group : forced_cta_group(),
               a->block_n, &cg, &bn, &rate);
     ProfScope prof(PROF_GEMM, stream, a->M + (a1 ? a1->M : 0), a->N, a->K, a->epilogue | ((bn >> 5) << 8) | (cg << 16));
     Problem g0, g1;
@@ -334,7 +349,8 @@ int launch_conv_inst(const CUtensorMap& ta, const CUtensorMap& tb, const GemmPar
     int grid = num_sms();
     if (tiles < grid) grid = tiles;
     GemmParams none{};
-    cudaError_t e = launch_pdl(kern, dim3(grid), dim3(kGemmThreads), (size_t)Cfg::kSmemBytes, st, 1, ta, tb, p, ta, tb, none, StreamKParams{nullptr, nullptr, 0, 0});
+    cudaError_t e = launch_pdl(kern, dim3(grid), dim3(kGemmThreads), (size_t)Cfg::kSmemBytes, st, 1, ta, tb, p, ta, tb, none, StreamKParams{nullptr, nullptr, 0, 0},
+                               ta, tb, ta, tb);
     if (e != cudaSuccess) return set_error("conv3x3 launch: %s", cudaGetErrorString(e));
     count_launch();
     return 0;

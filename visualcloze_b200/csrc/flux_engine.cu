@@ -8,6 +8,7 @@
 //   cat  [B, L, H + mlp]   columns [0,H): attention output; [H,H+mlp): GELU(mlp-up)  == linear2 input (layers.py:244)
 //   rope [64][B*L] float2 (pair-major), txt0 [B, Lt, H] (txt_in output), modulation tables for all evaluations.
 // Step-invariant work is hoisted into vcb_flux_prepare (SURVEY.md 7.5).
+#include <algorithm>
 #include <vector>
 
 #include "../../include/vcb200.h"
@@ -44,6 +45,10 @@ struct vcb_flux {
     void* sp_cat[VCB_SP_MAX] = {};
     int32_t* sp_flags[VCB_SP_MAX] = {};
     int32_t* sp_err = nullptr;
+    // unmerged LoRA: the largest rank of the Linears that carry one (0 = every Linear merged) and the down-projection buffer
+    // T [max(B * L, E * B), lora_rmax] bf16, written by each LoRA Linear's down-projection and read by its k-tail right after
+    int lora_rmax = 0;
+    uint16_t* lora_t = nullptr;
 };
 
 namespace {
@@ -85,6 +90,7 @@ int64_t carve(vcb_flux* f, uint8_t* base, int B, int Li, int Lt, int E) {
     uint8_t* cat8 = cv.take<uint8_t>(f->fp8 >= 2 ? (int64_t)B * L * (H + f->cfg.mlp_hidden) : 0);
     float* cat_scale = cv.take<float>(f->fp8 >= 2 ? (int64_t)B * L : 0);
     float* row_stats = cv.take<float>((int64_t)B * L * (H / 64) * 2);
+    uint16_t* lora_t = cv.take<uint16_t>(f->lora_rmax ? std::max<int64_t>((int64_t)B * L, EB) * f->lora_rmax : 0);
     // sequence-parallel: qkv [W*L, 3H/W] and cat [L, H+mlp] are the caller's peer-mapped allocations (same sizes)
     const bool sp = f->sp_world > 1;
     uint16_t* qkv = sp ? static_cast<uint16_t*>(f->sp_qkv[f->sp_rank]) : cv.take<uint16_t>((int64_t)B * L * 3 * H);
@@ -93,13 +99,45 @@ int64_t carve(vcb_flux* f, uint8_t* base, int B, int Li, int Lt, int E) {
         f->rope = rope; f->txt0 = txt0; f->temb_t = temb_t; f->temb_g = temb_g; f->h1 = h1; f->e_time = e_time;
         f->e_guid = e_guid; f->e_vec = e_vec; f->vec = vec; f->svec = svec; f->mod_dbl = md; f->mod_sgl = ms;
         f->mod_final = mod_final; f->x = x; f->xm = xm; f->qkv = qkv; f->cat = cat; f->xm8 = xm8; f->row_scale = row_scale; f->row_stats = row_stats;
-        f->cat8 = cat8; f->cat_scale = cat_scale;
+        f->cat8 = cat8; f->cat_scale = cat_scale; f->lora_t = lora_t;
     }
     return cv.off;
 }
 
+bool has_lora(const vcb_linear_w& w) { return w.rank > 0 && w.lora_scale != 0.f; }
+
+// One Linear, or two (the img and txt streams of a double block) in one grouped launch.  An unmerged LoRA Linear first runs its
+// down-projection T = bf16(s * A lora_a^T) into the T buffer, at the rows the main GEMM writes (the joint-row mapping of its A
+// operand; both streams' down-projections share one grouped launch), then the main GEMM reads T back through its LoRA k-tail.
+int gemm_linear(const vcb_flux* f, vcb_gemm_args* g, const vcb_linear_w* const* w, int n, void* stream) {
+    if (has_lora(*w[0]) || (n == 2 && has_lora(*w[1]))) {
+        vcb_gemm_args d[2];
+        for (int s = 0; s < n; ++s) {
+            const int r = w[s]->rank;
+            d[s] = vcb_gemm_args{};
+            d[s].M = g[s].M; d[s].N = r; d[s].K = g[s].K;
+            d[s].A = g[s].A; d[s].lda = g[s].lda; d[s].a_batch_stride = g[s].a_batch_stride;
+            d[s].W = w[s]->lora_a; d[s].ldw = g[s].K;
+            d[s].out = f->lora_t; d[s].ldo = r;
+            d[s].rows_per_batch = g[s].rows_per_batch; d[s].out_batch_rows = g[s].out_batch_rows; d[s].out_row_offset = g[s].out_row_offset;
+            d[s].epilogue = VCB_EPI_BIAS;
+            d[s].alpha = w[s]->lora_scale;
+            g[s].lora_t = f->lora_t + (int64_t)g[s].out_row_offset * r; g[s].ld_lora_t = r;
+            g[s].lora_t_batch_stride = (int64_t)g[s].out_batch_rows * r;
+            g[s].lora_b = w[s]->lora_b; g[s].lora_rank = r;
+        }
+        if (int rc = n == 2 ? vcb_gemm_bf16_grouped(&d[0], &d[1], stream) : vcb_gemm_bf16(&d[0], stream)) return rc;
+    }
+    return n == 2 ? vcb_gemm_bf16_grouped(&g[0], &g[1], stream) : vcb_gemm_bf16(&g[0], stream);
+}
+
+int gemm_linear(const vcb_flux* f, vcb_gemm_args& g, const vcb_linear_w& w, void* stream) {
+    const vcb_linear_w* wp = &w;
+    return gemm_linear(f, &g, &wp, 1, stream);
+}
+
 // plain [M,K] x [N,K]^T GEMM through the public entry point
-int linear(const void* A, int64_t lda, int M, int K, const vcb_linear_w& w, int N, void* out, int64_t ldo, int epi,
+int linear(const vcb_flux* f, const void* A, int64_t lda, int M, int K, const vcb_linear_w& w, int N, void* out, int64_t ldo, int epi,
            void* stream) {
     vcb_gemm_args g{};
     g.M = M; g.N = N; g.K = K;
@@ -108,7 +146,7 @@ int linear(const void* A, int64_t lda, int M, int K, const vcb_linear_w& w, int 
     g.out = out; g.ldo = ldo;
     g.rows_per_batch = M; g.out_batch_rows = M;
     g.epilogue = epi;
-    return vcb_gemm_bf16(&g, stream);
+    return gemm_linear(f, g, w, stream);
 }
 
 }  // namespace
@@ -122,8 +160,25 @@ extern "C" int vcb_flux_create(const vcb_flux_config* cfg, const vcb_flux_weight
         return set_error("flux_create: channel counts must be multiples of 8 (mlp_hidden of 128)");
     if (cfg->depth < 0 || cfg->depth_single < 0 || (cfg->depth && !w->dbl) || (cfg->depth_single && !w->sgl))
         return set_error("flux_create: missing block weights");
+    // unmerged LoRA Linears: validate, and size the down-projection buffer by the largest rank
+    int rmax = 0;
+    std::vector<const vcb_linear_w*> all = {&w->img_in, &w->txt_in, &w->time_in0, &w->time_in1, &w->vector_in0, &w->vector_in1,
+                                            &w->final_mod, &w->final_linear};
+    if (cfg->guidance_embed) { all.push_back(&w->guidance_in0); all.push_back(&w->guidance_in1); }
+    for (int i = 0; i < cfg->depth; ++i)
+        for (const vcb_stream_w* s : {&w->dbl[i].img, &w->dbl[i].txt})
+            for (const vcb_linear_w* l : {&s->mod, &s->qkv, &s->proj, &s->mlp0, &s->mlp2}) all.push_back(l);
+    for (int i = 0; i < cfg->depth_single; ++i)
+        for (const vcb_linear_w* l : {&w->sgl[i].mod, &w->sgl[i].linear1, &w->sgl[i].linear2}) all.push_back(l);
+    for (const vcb_linear_w* l : all) {
+        if (l->rank < 0 || l->rank % 8) return set_error("flux_create: LoRA rank %d must be a non-negative multiple of 8", l->rank);
+        if (!has_lora(*l)) continue;
+        if (!l->lora_a || !l->lora_b) return set_error("flux_create: an unmerged LoRA Linear (rank > 0) needs lora_a and lora_b");
+        rmax = std::max(rmax, (int)l->rank);
+    }
     vcb_flux* f = new vcb_flux();
     f->cfg = *cfg;
+    f->lora_rmax = rmax;
     f->w = *w;
     f->dbl.assign(w->dbl, w->dbl + cfg->depth);
     f->sgl.assign(w->sgl, w->sgl + cfg->depth_single);
@@ -140,6 +195,7 @@ extern "C" int vcb_flux_set_fp8(vcb_flux* f, int32_t level) {
     if (level < VCB_FP8_OFF || level > VCB_FP8_ALL_LINEARS) return set_error("flux_set_fp8: level must be 0 (off), 1 (LayerNorm-fed Linears) or 2 (all block Linears)");
     if (level) {
         if (f->sp_world > 1) return set_error("flux_set_fp8: the sequence-parallel mode runs bf16 projections");
+        if (f->lora_rmax) return set_error("flux_set_fp8: unmerged LoRA Linears run on bf16 operands (merge the LoRA weights for fp8)");
         auto has8 = [](const vcb_linear_w& w) { return w.w8 && w.w8_scale; };
         for (const auto& d : f->dbl)
             for (const vcb_stream_w* s : {&d.img, &d.txt}) {
@@ -191,6 +247,7 @@ extern "C" int vcb_flux_sp_attach(vcb_flux* f, int32_t world, int32_t rank, void
         return set_error("flux_sp_attach: bad arguments (world <= %d)", VCB_SP_MAX);
     if (f->cfg.heads % world) return set_error("flux_sp_attach: heads (%d) must be a multiple of world (%d)", f->cfg.heads, world);
     if (f->fp8) return set_error("flux_sp_attach: the sequence-parallel mode runs bf16 projections (switch vcb_flux_set_fp8 off first)");
+    if (f->lora_rmax) return set_error("flux_sp_attach: the sequence-parallel mode takes merged LoRA weights only");
     for (int r = 0; r < world; ++r) {
         if (!qkv[r] || !cat[r] || !flags[r]) return set_error("flux_sp_attach: null buffer for rank %d", r);
         f->sp_qkv[r] = qkv[r]; f->sp_cat[r] = cat[r]; f->sp_flags[r] = flags[r];
@@ -219,32 +276,32 @@ extern "C" int vcb_flux_prepare(vcb_flux* f, void* workspace, int64_t workspace_
     // RoPE table (constant across steps; the reference recomputes it per call, model.py:110-111)
     if ((rc = vcb_rope_table(ids, f->rope, B * f->L, c.axes_dim[0], c.axes_dim[1], c.axes_dim[2], c.theta, stream))) return rc;
     // txt_in (constant across steps, model.py:108)
-    if ((rc = linear(txt, c.context_in_dim, B * Lt, c.context_in_dim, f->w.txt_in, H, f->txt0, H, VCB_EPI_BIAS, stream))) return rc;
+    if ((rc = linear(f, txt, c.context_in_dim, B * Lt, c.context_in_dim, f->w.txt_in, H, f->txt0, H, VCB_EPI_BIAS, stream))) return rc;
     // vec for every evaluation (model.py:102-107)
     if ((rc = vcb_timestep_embedding(t_scaled, freqs, f->temb_t, EB, stream))) return rc;
-    if ((rc = linear(f->temb_t, 256, EB, 256, f->w.time_in0, H, f->h1, H, VCB_EPI_BIAS, stream))) return rc;
+    if ((rc = linear(f, f->temb_t, 256, EB, 256, f->w.time_in0, H, f->h1, H, VCB_EPI_BIAS, stream))) return rc;
     if ((rc = vcb_silu(f->h1, f->h1, (int64_t)EB * H, stream))) return rc;
-    if ((rc = linear(f->h1, H, EB, H, f->w.time_in1, H, f->e_time, H, VCB_EPI_BIAS, stream))) return rc;
+    if ((rc = linear(f, f->h1, H, EB, H, f->w.time_in1, H, f->e_time, H, VCB_EPI_BIAS, stream))) return rc;
     if (c.guidance_embed) {
         if ((rc = vcb_timestep_embedding(g_scaled, freqs, f->temb_g, B, stream))) return rc;
-        if ((rc = linear(f->temb_g, 256, B, 256, f->w.guidance_in0, H, f->h1, H, VCB_EPI_BIAS, stream))) return rc;
+        if ((rc = linear(f, f->temb_g, 256, B, 256, f->w.guidance_in0, H, f->h1, H, VCB_EPI_BIAS, stream))) return rc;
         if ((rc = vcb_silu(f->h1, f->h1, (int64_t)B * H, stream))) return rc;
-        if ((rc = linear(f->h1, H, B, H, f->w.guidance_in1, H, f->e_guid, H, VCB_EPI_BIAS, stream))) return rc;
+        if ((rc = linear(f, f->h1, H, B, H, f->w.guidance_in1, H, f->e_guid, H, VCB_EPI_BIAS, stream))) return rc;
     }
-    if ((rc = linear(y, c.vec_in_dim, B, c.vec_in_dim, f->w.vector_in0, H, f->h1, H, VCB_EPI_BIAS, stream))) return rc;
+    if ((rc = linear(f, y, c.vec_in_dim, B, c.vec_in_dim, f->w.vector_in0, H, f->h1, H, VCB_EPI_BIAS, stream))) return rc;
     if ((rc = vcb_silu(f->h1, f->h1, (int64_t)B * H, stream))) return rc;
-    if ((rc = linear(f->h1, H, B, H, f->w.vector_in1, H, f->e_vec, H, VCB_EPI_BIAS, stream))) return rc;
+    if ((rc = linear(f, f->h1, H, B, H, f->w.vector_in1, H, f->e_vec, H, VCB_EPI_BIAS, stream))) return rc;
     if ((rc = vcb_add3(f->e_time, c.guidance_embed ? f->e_guid : nullptr, B, f->e_vec, B, f->vec, EB, H, stream))) return rc;
     if ((rc = vcb_silu(f->vec, f->svec, (int64_t)EB * H, stream))) return rc;
     // AdaLN modulation vectors of all evaluations: one GEMM per block reads each modulation weight once per image
     // instead of once per step (layers.py:121 is a GEMV re-reading 6.5 GB per step in the reference)
     for (int i = 0; i < c.depth; ++i) {
-        if ((rc = linear(f->svec, H, EB, H, f->dbl[i].img.mod, 6 * H, f->mod_dbl[2 * i], 6 * H, VCB_EPI_BIAS, stream))) return rc;
-        if ((rc = linear(f->svec, H, EB, H, f->dbl[i].txt.mod, 6 * H, f->mod_dbl[2 * i + 1], 6 * H, VCB_EPI_BIAS, stream))) return rc;
+        if ((rc = linear(f, f->svec, H, EB, H, f->dbl[i].img.mod, 6 * H, f->mod_dbl[2 * i], 6 * H, VCB_EPI_BIAS, stream))) return rc;
+        if ((rc = linear(f, f->svec, H, EB, H, f->dbl[i].txt.mod, 6 * H, f->mod_dbl[2 * i + 1], 6 * H, VCB_EPI_BIAS, stream))) return rc;
     }
     for (int i = 0; i < c.depth_single; ++i)
-        if ((rc = linear(f->svec, H, EB, H, f->sgl[i].mod, 3 * H, f->mod_sgl[i], 3 * H, VCB_EPI_BIAS, stream))) return rc;
-    if ((rc = linear(f->svec, H, EB, H, f->w.final_mod, 2 * H, f->mod_final, 2 * H, VCB_EPI_BIAS, stream))) return rc;
+        if ((rc = linear(f, f->svec, H, EB, H, f->sgl[i].mod, 3 * H, f->mod_sgl[i], 3 * H, VCB_EPI_BIAS, stream))) return rc;
+    if ((rc = linear(f, f->svec, H, EB, H, f->w.final_mod, 2 * H, f->mod_final, 2 * H, VCB_EPI_BIAS, stream))) return rc;
     f->prepared = true;
     return 0;
 }
@@ -330,7 +387,7 @@ int stream_gemm(const vcb_flux* f, const StreamView& sv, const uint16_t* a_buf, 
     (void)qk;
     vcb_gemm_args g = stream_args(f, sv, a_buf, lda, a_col, K, w, N, epi, out, ldo, out_col, gate, gate_stride, q_scale, k_scale,
                                   out2, ldo2, out2_col);
-    return vcb_gemm_bf16(&g, stream);
+    return gemm_linear(f, g, w, stream);
 }
 
 // fp8: the LayerNorm feeds an fp8 projection -> e4m3 rows + per-row scales instead of bf16 rows
@@ -402,7 +459,7 @@ extern "C" int vcb_flux_forward(vcb_flux* f, int32_t e, const void* img, int64_t
         g.out = f->x; g.ldo = H;
         g.rows_per_batch = Li; g.out_batch_rows = L; g.out_row_offset = Lt;
         g.epilogue = VCB_EPI_BIAS;
-        if ((rc = vcb_gemm_bf16(&g, stream))) return rc;
+        if ((rc = gemm_linear(f, g, f->w.img_in, stream))) return rc;
     }
     for (int b = 0; b < B; ++b) {
         cudaError_t ce = cudaMemcpyAsync(f->x + (int64_t)b * L * H, f->txt0 + (int64_t)b * Lt * H, (size_t)Lt * H * 2,
@@ -421,36 +478,40 @@ extern "C" int vcb_flux_forward(vcb_flux* f, int32_t e, const void* img, int64_t
         if ((rc = double_ln(f, sv, mod, 0, stream))) return rc;
         {
             vcb_gemm_args g[2];
+            const vcb_linear_w* lw[2] = {&sw[0]->qkv, &sw[1]->qkv};
             for (int s = 0; s < 2; ++s)
                 g[s] = stream_args(f, *sv[s], f->xm, H, 0, H, sw[s]->qkv, 3 * H, VCB_EPI_QKV, f->qkv, 3 * H, 0, nullptr, 0,
                                    sw[s]->q_scale, sw[s]->k_scale, nullptr, 0, 0);
-            if ((rc = vcb_gemm_bf16_grouped(&g[0], &g[1], stream))) return rc;
+            if ((rc = gemm_linear(f, g, lw, 2, stream))) return rc;
         }
         if ((rc = joint_attention(f, ldc, w.attn_score_bound, stream))) return rc;
         if ((rc = quantize_cat(f, ldc, 0, H, stream))) return rc;
         {
             vcb_gemm_args g[2];
+            const vcb_linear_w* lw[2] = {&sw[0]->proj, &sw[1]->proj};
             for (int s = 0; s < 2; ++s)
                 g[s] = stream_args(f, *sv[s], f->cat, ldc, 0, H, sw[s]->proj, H, VCB_EPI_GATE_RES, f->x, H, 0, mod[s] + 2 * H, 6 * H,
                                    nullptr, nullptr, nullptr, 0, 0);
-            if ((rc = vcb_gemm_bf16_grouped(&g[0], &g[1], stream))) return rc;
+            if ((rc = gemm_linear(f, g, lw, 2, stream))) return rc;
             f->stats_valid = true;             // both streams' rows of x now have their LayerNorm statistics in row_stats
         }
         if ((rc = double_ln(f, sv, mod, 3 * H, stream))) return rc;
         {
             vcb_gemm_args g[2];
+            const vcb_linear_w* lw[2] = {&sw[0]->mlp0, &sw[1]->mlp0};
             for (int s = 0; s < 2; ++s)
                 g[s] = stream_args(f, *sv[s], f->xm, H, 0, H, sw[s]->mlp0, mlp, VCB_EPI_BIAS_GELU, f->cat, ldc, H, nullptr, 0, nullptr,
                                    nullptr, nullptr, 0, 0);
-            if ((rc = vcb_gemm_bf16_grouped(&g[0], &g[1], stream))) return rc;
+            if ((rc = gemm_linear(f, g, lw, 2, stream))) return rc;
         }
         if ((rc = quantize_cat(f, ldc, H, mlp, stream))) return rc;
         {
             vcb_gemm_args g[2];
+            const vcb_linear_w* lw[2] = {&sw[0]->mlp2, &sw[1]->mlp2};
             for (int s = 0; s < 2; ++s)
                 g[s] = stream_args(f, *sv[s], f->cat, ldc, H, mlp, sw[s]->mlp2, H, VCB_EPI_GATE_RES, f->x, H, 0, mod[s] + 5 * H, 6 * H,
                                    nullptr, nullptr, nullptr, 0, 0);
-            if ((rc = vcb_gemm_bf16_grouped(&g[0], &g[1], stream))) return rc;
+            if ((rc = gemm_linear(f, g, lw, 2, stream))) return rc;
             f->stats_valid = true;
         }
     }
@@ -478,7 +539,7 @@ extern "C" int vcb_flux_forward(vcb_flux* f, int32_t e, const void* img, int64_t
         g.out = out; g.ldo = ld_out;
         g.rows_per_batch = Li; g.out_batch_rows = Li; g.out_row_offset = 0;
         g.epilogue = VCB_EPI_BIAS;
-        if ((rc = vcb_gemm_bf16(&g, stream))) return rc;
+        if ((rc = gemm_linear(f, g, f->w.final_linear, stream))) return rc;
     }
     return 0;
 }

@@ -85,6 +85,12 @@ struct GemmParams {
     // The kernel's kSp instantiation writes each thread's 16-byte pieces through the peer-mapped pointers.
     int sp_world, sp_row_offset;
     __nv_bfloat16* sp_out[kSpMaxRanks];
+    // Unmerged LoRA k-tail (bf16 operands): acc = A W^T + T B_lora^T, i.e. [A | T] [W | B_lora]^T.  After the ceil(K / 64)
+    // k-blocks of (A, W) the producer loads ceil(lora_rank / 64) more from the T map (addressed like A: same rows_per_batch /
+    // batch mapping) and the B_lora map (boxed like W, multicast like W under cta_group 2).  0 = no tail.
+    int lora_rank;
+    // output scale: the epilogue sees alpha * acc (0 = 1) -- the LoRA down-projection T = bf16(s * X A^T)
+    float alpha;
 };
 
 // Stream-K tail (optional): the tiles of the partial last wave are cut along K into one equal contiguous range per CTA
@@ -188,7 +194,9 @@ template <int BLOCK_N, int kCtaGroup, int kEpi, int kAMode = A_MATRIX, bool kSp 
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const GemmParams p,
                   const __grid_constant__ CUtensorMap tmap_a1, const __grid_constant__ CUtensorMap tmap_b1, const GemmParams p1,
-                  const StreamKParams skp) {
+                  const StreamKParams skp,
+                  const __grid_constant__ CUtensorMap tmap_t, const __grid_constant__ CUtensorMap tmap_lb,
+                  const __grid_constant__ CUtensorMap tmap_t1, const __grid_constant__ CUtensorMap tmap_lb1) {
     static_assert(!kSp || kEpi == EPI_QKV || kEpi == EPI_LINEAR1, "sequence-parallel routing lives in the head-structured epilogues");
     static_assert(!kFp8 || (kAMode == A_MATRIX && !kSp), "fp8 operands: plain matrices, single-GPU path");
     static_assert(kAMode == A_MATRIX || kCtaGroup == 1, "conv mode is single-CTA");
@@ -218,6 +226,14 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
             tma_prefetch_desc(&tmap_a1);
             tma_prefetch_desc(&tmap_b1);
         }
+        if (!kFp8 && kAMode == A_MATRIX && p.lora_rank > 0) {
+            tma_prefetch_desc(&tmap_t);
+            tma_prefetch_desc(&tmap_lb);
+            if (p1.batch > 0) {
+                tma_prefetch_desc(&tmap_t1);
+                tma_prefetch_desc(&tmap_lb1);
+            }
+        }
         for (int s = 0; s < kStages; ++s) {
             mbar_init(&full_bar[s], 1);
             mbar_init(&empty_bar[s], 2 * kCtaGroup);      // one arrive per consumer warpgroup of every CTA the stage was sent to
@@ -237,7 +253,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     const int m_per_sample1 = (p1.rows_per_batch + tile_m - 1) / tile_m;
     const int num_m1 = p1.batch > 0 ? m_per_sample1 * p1.batch : 0;
     const int num_tiles = tiles0 + num_m1 * num_n;
-    const int num_kb = (p.K + kBlockKEl - 1) / kBlockKEl;
+    // the LoRA k-tail adds its k-blocks behind the main ones, so the stream-K split and the grouped launch cover it unchanged
+    // (both problems of a grouped launch share K and lora_rank)
+    const int kb_main = (p.K + kBlockKEl - 1) / kBlockKEl;
+    const int num_kb = kb_main + ((!kFp8 && kAMode == A_MATRIX) ? (p.lora_rank + kBlockK - 1) / kBlockK : 0);
     const int cluster_id = blockIdx.x / kCtaGroup;
     const int num_clusters = gridDim.x / kCtaGroup;
 
@@ -262,6 +281,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
                 for (int kb = kb0; kb < kb1; ++kb) {
                     mbar_wait(&empty_bar[stage], phase ^ 1);
                     mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
+                    const bool tail = kb >= kb_main;       // LoRA k-tail: T in place of A, B_lora in place of W
+                    const int kc = (tail ? kb - kb_main : kb) * kBlockKEl;
                     if constexpr (kAMode == A_CONV3X3) {
                         const int cpb = p.conv_C / kBlockK;
                         const int tap = kb / cpb, cb = kb - tap * cpb;
@@ -271,10 +292,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
                         const int y0 = (mi / conv_tx) * kConvTileH * p.conv_stride + (tap / 3) - pad;
                         tma_load_4d(ta, &full_bar[stage], smem_a + stage * Cfg::kABytes, cb * kBlockK, x0, y0, bi, kEvictNormal);
                     } else {
-                        tma_load_3d(ta, &full_bar[stage], smem_a + stage * Cfg::kABytes, kb * kBlockKEl, m0, bi, hint_a);
+                        tma_load_3d(tail ? (g1 ? &tmap_t1 : &tmap_t) : ta, &full_bar[stage], smem_a + stage * Cfg::kABytes, kc, m0, bi, hint_a);
                     }
-                    tma_load_2d<kCtaGroup == 2>(tb, &full_bar[stage], smem_b + stage * Cfg::kBBytes + (int)cta_rank * Cfg::kBRows * 128,
-                                                kb * kBlockKEl, n0, hint_b, (uint16_t)3);
+                    tma_load_2d<kCtaGroup == 2>(tail ? (g1 ? &tmap_lb1 : &tmap_lb) : tb, &full_bar[stage],
+                                                smem_b + stage * Cfg::kBBytes + (int)cta_rank * Cfg::kBRows * 128, kc, n0, hint_b, (uint16_t)3);
                     if (++stage == kStages) { stage = 0; phase ^= 1; }
                 }
             }
@@ -348,6 +369,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
 #pragma unroll
                     for (int i = 0; i < kAccRegs; ++i) acc[i] += __ldcg(part + i * kGemmConsumers);
                 }
+            }
+            if (P.alpha != 0.f && P.alpha != 1.f) {
+#pragma unroll
+                for (int i = 0; i < kAccRegs; ++i) acc[i] *= P.alpha;
             }
 
             // ---------------- epilogue: this thread's two rows (h = 0, 1: frag_row + 8 h) ----------------

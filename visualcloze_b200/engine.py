@@ -1,8 +1,10 @@
 """Host-side driver of the FLUX-DiT engine in libvcb200 (vcb_flux_* in include/vcb200.h).
 
-Packs the reference's parameters (LoRA merged), owns the device workspace, and marshals pointers.  Arithmetic
-done here in torch is limited to one-off weight packing (``W + s * B @ A`` at load time) and scalar/host
-bookkeeping (time grids, masks -> sequence lengths); every per-token operation of the path runs in the library.
+Packs the reference's parameters, owns the device workspace, and marshals pointers.  LoRA is either merged (``W + s * B @ A``
+formed once at packing time, a second copy of the weights) or unmerged (the engine points at the module's own ``W``, ``A``
+and ``B``; every call adds ``s * (x A^T) B^T`` in the GEMM's k-tail).  Arithmetic done here in torch is limited to that one-off
+packing and scalar/host bookkeeping (time grids, masks -> sequence lengths); every per-token operation of the path runs in
+the library.
 """
 from __future__ import annotations
 
@@ -25,7 +27,14 @@ def _freqs() -> Tensor:
 
 
 class FluxEngine:
-    def __init__(self, params, named_params: dict[str, Tensor], lora_scale: float = 1.0, fp8: int = 0):
+    def __init__(self, params, named_params: dict[str, Tensor], lora_scale: float = 1.0, fp8: int = 0, lora_mode: str = "merged",
+                 workspace: Tensor | None = None):
+        """``lora_mode``: "merged" or "unmerged" (see the module docstring; unmerged takes bf16 projections only).
+        ``workspace``: a previous engine's device workspace to reuse (grown on demand by ``prepare``)."""
+        if lora_mode not in ("merged", "unmerged"):
+            raise ValueError("lora_mode must be 'merged' or 'unmerged'")
+        if lora_mode == "unmerged" and fp8:
+            raise ValueError("unmerged LoRA runs on bf16 operands; the fp8 projections need merged weights")
         some = next(iter(named_params.values()))
         if not some.is_cuda:
             raise _lib.VcbError("FluxEngine needs the model on a CUDA device: the hot path has no CPU fallback")
@@ -36,11 +45,12 @@ class FluxEngine:
         self._p = named_params
         self._scale = float(lora_scale)
         self.fp8 = int(fp8)                    # 0 = bf16, 1 = LayerNorm-fed Linears on e4m3, 2 = every block Linear on e4m3
+        self.lora_mode = lora_mode
         self.H = params.hidden_size
         self.mlp = int(params.hidden_size * params.mlp_ratio)
         with torch.no_grad():
             self._build()
-        self._ws = None
+        self._ws = workspace
         self._shape = None
         self._sp = None
         self._freqs = _freqs().to(self.device)
@@ -49,6 +59,8 @@ class FluxEngine:
     def enable_sequence_parallel(self, sp) -> None:
         """``sp``: a ``parallel.SequenceParallel`` (or None to switch back).  Every rank then passes the FULL txt / ids to
         ``prepare`` (identical on all ranks) and its LOCAL img rows (``sp.shard``) to ``forward``."""
+        if sp is not None and sp.world > 1 and self.lora_mode == "unmerged":
+            raise ValueError("sequence-parallel mode takes merged LoRA weights only")
         if sp is not None and self.params.num_heads % sp.world:
             raise ValueError(f"num_heads ({self.params.num_heads}) must be a multiple of the sequence-parallel world size ({sp.world})")
         if sp is None and self._sp is not None:
@@ -65,6 +77,8 @@ class FluxEngine:
         w = p[name + ".weight"]
         a = p.get(name + ".lora_A.weight")
         b = p.get(name + ".bias")
+        if self.lora_mode == "unmerged":
+            return self._linear_unmerged(name, w, a, b)
         w32 = None
         if a is not None:
             # merged LoRA (lora.py:92-98): W' = W + s * B A in fp32, rounded once to bf16
@@ -80,13 +94,32 @@ class FluxEngine:
             w8 = (w32 / w8s[:, None]).to(torch.float8_e4m3fn).contiguous()
             self._keep += [w8, w8s]
         del w32
-        bias = torch.zeros(w.shape[0], dtype=torch.float32, device=w.device) if b is None else b.float()
-        bb = p.get(name + ".lora_B.bias")
+        bias = self._bias(name, b, w.shape[0])
+        self._keep.append(w)
+        return LinearW(w.data_ptr(), bias.data_ptr(), 0 if w8 is None else w8.data_ptr(), 0 if w8s is None else w8s.data_ptr())
+
+    def _bias(self, name: str, b: Tensor | None, n: int) -> Tensor:
+        """fp32 bias of the packed Linear: ``b + s * b_B`` (lora.py:92-98)."""
+        bias = torch.zeros(n, dtype=torch.float32, device=self.device) if b is None else b.float()
+        bb = self._p.get(name + ".lora_B.bias")
         if bb is not None:
             bias = bias + self._scale * bb.float()
         bias = bias.contiguous()
-        self._keep += [w, bias]
-        return LinearW(w.data_ptr(), bias.data_ptr(), 0 if w8 is None else w8.data_ptr(), 0 if w8s is None else w8s.data_ptr())
+        self._keep.append(bias)
+        return bias
+
+    def _linear_unmerged(self, name: str, w: Tensor, a: Tensor | None, b: Tensor | None) -> LinearW:
+        """Unmerged LoRA: the module's own bf16 ``weight``, ``lora_A`` [r, in] and ``lora_B`` [out, r] (no copy when they are bf16
+        and contiguous, as FluxLoraWrapper's parameters are); only the fp32 bias ``b + s * b_B`` is formed here."""
+        w = w.to(BF16).contiguous()
+        self._keep.append(w)
+        bias = self._bias(name, b, w.shape[0])
+        if a is None:
+            return LinearW(w.data_ptr(), bias.data_ptr(), 0, 0, 0, 0, 0, 0.0)
+        a = a.to(BF16).contiguous()
+        lb = self._p[name + ".lora_B.weight"].to(BF16).contiguous()
+        self._keep += [a, lb]
+        return LinearW(w.data_ptr(), bias.data_ptr(), 0, 0, a.data_ptr(), lb.data_ptr(), a.shape[0], self._scale)
 
     def _scale_vec(self, name: str) -> int:
         t = self._p[name].to(BF16).contiguous()

@@ -9,8 +9,11 @@ Mirror of ``models/model.py`` (``FluxParams`` :18-32, ``Flux`` :35-151, ``FluxLo
     ``double_blocks.{i}.img_attn.qkv.lora_A.weight`` ...; SURVEY.md 8b "Weights"), so BFL safetensors and the
     LoRA checkpoint load with the reference's own ``load_state_dict(..., strict=False)`` sequence
     (``visualcloze.py:111-112``);
-  * ``FluxLoraWrapper.set_lora_scale`` keeps its meaning; LoRA is merged into the packed weights
-    (``W' = W + s * B A``, ``b' = b + s * b_B``), re-packed when the scale or a parameter changes.
+  * ``FluxLoraWrapper.set_lora_scale`` keeps its meaning.  By default LoRA is merged into packed weights
+    (``W' = W + s * B A``, ``b' = b + s * b_B``), re-packed when the scale or a parameter changes: a second copy of
+    the weights.  ``set_lora_mode("unmerged")`` runs it as the reference does, ``base(x) + s * B(A(x))``, on the
+    module's own tensors: a scale change or an adapter swap (``load_state_dict(sd, strict=False, assign=True)``)
+    then only rebuilds pointers and bias vectors, at about 8 % more GEMM work per evaluation.
 
 The module holds parameters only; all arithmetic happens in the CUDA library (``engine.py``).  There is no
 PyTorch fallback: calling ``forward`` without an H100 raises.
@@ -123,6 +126,8 @@ class Flux(nn.Module):
         # are allocated with torch.empty, and packing an engine from never-loaded memory must fail loudly, not render garbage
         self._initialized: set[str] = set()
         self.linear_precision = "bf16"
+        self.lora_mode = "merged"
+        self._sp = None
         kw = dict(device=device, dtype=dtype)
         for name, fin, fout in linear_table(params):
             _attach(self, name + ".weight", nn.Parameter(torch.empty(fout, fin, **kw), requires_grad=False))
@@ -178,10 +183,13 @@ class Flux(nn.Module):
             from ._lib import VcbError
             raise VcbError(f"{len(missing)} base parameters were never loaded (e.g. {missing[:3]}): load the FLUX.1-Fill checkpoint "
                            "(VisualClozeModel(flux_ckpt=...) / load_state_dict) or call init_synthetic() before running the model")
-        key = (self.lora_scale, self.linear_precision) + tuple((p.data_ptr(), p._version) for p in self.parameters())
+        key = (self.lora_scale, self.linear_precision, self.lora_mode) + tuple((p.data_ptr(), p._version) for p in self.parameters())
         if self._engine is None or key != self._packed_key:
+            ws = self._engine._ws if self._engine is not None else None     # the device workspace carries over
             self._engine = None                     # release the previous packing before building the next one
-            self._engine = FluxEngine(self.params, dict(self.named_parameters()), self.lora_scale, fp8={"bf16": 0, "fp8": 1, "fp8_all": 2}[self.linear_precision])
+            self._engine = FluxEngine(self.params, dict(self.named_parameters()), self.lora_scale,
+                                      fp8={"bf16": 0, "fp8": 1, "fp8_all": 2}[self.linear_precision], lora_mode=self.lora_mode,
+                                      workspace=ws)
             self._packed_key = key
             if getattr(self, "_sp", None) is not None:
                 self._engine.enable_sequence_parallel(self._sp)
@@ -195,12 +203,32 @@ class Flux(nn.Module):
         bf16 path (its own numbers in the same contract).  No counterpart in the reference."""
         if precision not in ("bf16", "fp8", "fp8_all"):
             raise ValueError("linear precision must be 'bf16', 'fp8' or 'fp8_all'")
+        if precision != "bf16" and self.lora_mode == "unmerged":
+            raise ValueError("the fp8 projections need merged LoRA weights (set_lora_mode('merged') first)")
         self.linear_precision = precision
+
+    def set_lora_mode(self, mode: str) -> None:
+        """"merged" (default): the engine packs ``W + s * B A`` once, a second copy of every weight, and re-merges when the scale
+        or a parameter changes.  "unmerged": every call computes ``base(x) + s * B(A(x))`` like the reference's LinearLora
+        (lora.py:92-98), on the module's own tensors; changing the scale or swapping adapters costs a bias rebuild, each
+        evaluation about 8 % more GEMM work.  Which is better depends on how often the adapter or scale changes and on how
+        much memory other resident models need.  Unmerged takes bf16 projections on one GPU: it refuses fp8 precisions and
+        sequence parallelism."""
+        if mode not in ("merged", "unmerged"):
+            raise ValueError("lora mode must be 'merged' or 'unmerged'")
+        if mode == "unmerged":
+            if self.linear_precision != "bf16":
+                raise ValueError("unmerged LoRA runs on bf16 operands (set_linear_precision('bf16') first)")
+            if self._sp is not None and self._sp.world > 1:
+                raise ValueError("sequence-parallel mode takes merged LoRA weights only")
+        self.lora_mode = mode
 
     def enable_sequence_parallel(self, sp) -> None:
         """Single-image latency mode over several GPUs (``parallel.SequenceParallel``; None switches it off).  No counterpart
         in the reference (single-GPU inference); the call signature and the results' contract are unchanged: every rank
-        passes the same full inputs and receives the same full output."""
+        passes the same full inputs and receives the same full output.  Needs merged LoRA weights."""
+        if sp is not None and sp.world > 1 and self.lora_mode == "unmerged":
+            raise ValueError("sequence-parallel mode takes merged LoRA weights only (set_lora_mode('merged') first)")
         self._sp = sp
         if self._engine is not None:
             self._engine.enable_sequence_parallel(sp)

@@ -51,10 +51,13 @@ def gemm_args(a: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None, out: 
          hidden: int = 0, q_scale=None, k_scale=None, rope=None, out2=None, out2_col_offset: int = 0,
          block_n: int = 0, cta_group: int = 0, a_batch_stride: int = 0, m: int | None = None,
          sp_out: list | None = None, sp_row_offset: int = 0, a_scale: torch.Tensor | None = None,
-         w_scale: torch.Tensor | None = None, row_stats: torch.Tensor | None = None):
+         w_scale: torch.Tensor | None = None, row_stats: torch.Tensor | None = None, lora_t: torch.Tensor | None = None,
+         lora_b: torch.Tensor | None = None, lora_t_batch_stride: int = 0, alpha: float = 0.0):
     """out[...] = epilogue(a @ w.T).  a [M,K], w [N,K], out 2-D (rows, ld); see include/vcb200.h.
     With batching (rows_per_batch < M) sample b's rows start at a + b * a_batch_stride (elements).
-    fp8: a and w of dtype ``torch.float8_e4m3fn`` (both), with ``a_scale`` [output rows] / ``w_scale`` [N] fp32."""
+    fp8: a and w of dtype ``torch.float8_e4m3fn`` (both), with ``a_scale`` [output rows] / ``w_scale`` [N] fp32.
+    LoRA k-tail: ``lora_t`` [rows, r] (addressed like ``a``, sample b at lora_t + b * lora_t_batch_stride) and ``lora_b`` [N, r]
+    bf16 add ``lora_t @ lora_b.T`` to the accumulator.  ``alpha``: output scale, the epilogue sees alpha * acc (0 = 1)."""
     fp8 = a.dtype == torch.float8_e4m3fn
     if fp8:
         _req(a, torch.float8_e4m3fn, "a"); _req(w, torch.float8_e4m3fn, "w")
@@ -105,7 +108,14 @@ def gemm_args(a: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None, out: 
         if w_scale is not None:
             _req(w_scale, torch.float32, "w_scale")
         g.a_scale, g.w_scale = _p(a_scale), _p(w_scale)
-    g._keepalive = (a, w, bias, out, gate, res, q_scale, k_scale, rope, out2, sp_out, a_scale, w_scale, row_stats)
+    if lora_t is not None or lora_b is not None:
+        _req(lora_t, BF16, "lora_t"); _req(lora_b, BF16, "lora_b")
+        if lora_b.stride(0) != lora_b.shape[1]:
+            raise _lib.VcbError("lora_b must be a dense [N, r] matrix")
+        g.lora_t, g.ld_lora_t, g.lora_t_batch_stride = lora_t.data_ptr(), lora_t.stride(0), lora_t_batch_stride
+        g.lora_b, g.lora_rank = lora_b.data_ptr(), lora_b.shape[1]
+    g.alpha = alpha
+    g._keepalive = (a, w, bias, out, gate, res, q_scale, k_scale, rope, out2, sp_out, a_scale, w_scale, row_stats, lora_t, lora_b)
     return g, out
 
 
