@@ -309,7 +309,8 @@ int  vcb_flux_use_score_bounds(vcb_flux* f, int32_t enable);
 #define VCB_FP8_ALL_LINEARS 2
 int  vcb_flux_set_fp8(vcb_flux* f, int32_t level);
 /* bytes of device workspace for B samples of Li image + Lt text tokens and n_evals model evaluations (with unmerged LoRA
- * Linears: + the down-projection buffer T [max(B * (Li + Lt), n_evals * B), largest rank] bf16) */
+ * Linears: + the down-projection buffer T [max(B * (Li + Lt), n_evals * B), largest rank] bf16; with the first-block cache on:
+ * + its buffers, vcb_flux_set_first_block_cache) */
 int64_t vcb_flux_workspace_bytes(const vcb_flux* f, int32_t B, int32_t Li, int32_t Lt, int32_t n_evals);
 /* Step-invariant work, once per image (SURVEY.md 2.2: txt_in, RoPE table, and the AdaLN modulation vectors of
  * all n_evals steps as one batched GEMM per block).  t_scaled: [n_evals * B] fp32 = 1000 * flux_time (row e*B+b);
@@ -323,6 +324,19 @@ int vcb_flux_prepare(vcb_flux* f, void* workspace, int64_t workspace_bytes, int3
  * img [B*Li, in_channels] bf16 (latent || cond) -> out [B*Li, out_channels] bf16. */
 int vcb_flux_forward(vcb_flux* f, int32_t eval_idx, const void* img, int64_t ld_img, void* out, int64_t ld_out,
                      void* stream);
+/* Opt-in first-block cache (FBCache; off by default; NOT the reference's numerics).  threshold > 0 switches it on, 0 off.  Per
+ * vcb_flux_prepare, evaluation k runs img_in and double block 0 as usual; with x0 / x1 the img rows of x before / after that
+ * block, r_k = bf16(x1 - x0) and diff_k = sum|r_k - r_ref| / sum|r_ref| (fp32, fixed summation order, valid img rows of every
+ * sample: right padding excluded through seqlens; one decision per batch).  k > 0 and diff_k < threshold: the img rows become
+ * bf16(x1 + R) and go straight to the final layer.  Otherwise blocks 1.. run, r_ref = r_k and R = x_final - x1 (fp32) are kept.
+ * The first evaluation after every prepare is computed.  While on, the final LayerNorm computes its own row statistics (also on
+ * computed evaluations), and vcb_flux_forward reads the decision on the host: it synchronises `stream` once per call and cannot be
+ * captured in a CUDA graph.  The workspace grows by B * Li * hidden * 8 bytes (x0 / r_ref bf16 pair + R fp32).  Refused in
+ * sequence-parallel mode (and vcb_flux_sp_attach refuses while it is on); needs depth >= 1. */
+int vcb_flux_set_first_block_cache(vcb_flux* f, float threshold);
+/* evaluations computed / skipped since the last vcb_flux_prepare, and diff of the latest one (+inf for the first evaluation after
+ * prepare, which has nothing to compare with; NaN before any) */
+int vcb_flux_cache_stats(const vcb_flux* f, int32_t* computed, int32_t* skipped, float* last_diff);
 
 /* ---- single-image sequence parallelism over NVLink peer memory (SURVEY.md 8f-2: the reference has no multi-GPU
  * inference; the join point is the attention call, layers.py:177-187 / 236-241) -----------------------------------

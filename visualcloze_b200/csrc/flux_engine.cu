@@ -9,9 +9,11 @@
 //   rope [64][B*L] float2 (pair-major), txt0 [B, Lt, H] (txt_in output), modulation tables for all evaluations.
 // Step-invariant work is hoisted into vcb_flux_prepare (SURVEY.md 7.5).
 #include <algorithm>
+#include <cmath>
 #include <vector>
 
 #include "../../include/vcb200.h"
+#include "fbcache.cuh"
 #include "host_util.cuh"
 
 using namespace vcb;
@@ -49,6 +51,19 @@ struct vcb_flux {
     // T [max(B * L, E * B), lora_rmax] bf16, written by each LoRA Linear's down-projection and read by its k-tail right after
     int lora_rmax = 0;
     uint16_t* lora_t = nullptr;
+    // first-block cache (vcb_flux_set_first_block_cache; threshold 0 = off).  fbc_buf[fbc_ref] holds r_ref, the block-0 residual
+    // of the last computed evaluation; the other one takes the x0 copy, which the decision turns into r_k in place -- a computed
+    // evaluation then swaps the two and parks x1 in the freed one until the residual R is stored
+    float fbc_threshold = 0.f;
+    uint16_t* fbc_buf[2] = {};        // [B * Li, H] bf16 each
+    int fbc_ref = 0;
+    float* fbc_R = nullptr;           // [B * Li, H] fp32: x_final - x1 of the last computed evaluation
+    float2* fbc_part = nullptr;       // [kFbcMaxBlocks] partial sums of the decision
+    float* fbc_res = nullptr;         // [4] num, den, diff, skip (device)
+    float* fbc_host = nullptr;        // [4] pinned copy read by the host
+    int32_t fbc_computed = 0, fbc_skipped = 0;
+    float fbc_last_diff = NAN;
+    ~vcb_flux() { if (fbc_host) cudaFreeHost(fbc_host); }
 };
 
 namespace {
@@ -91,6 +106,12 @@ int64_t carve(vcb_flux* f, uint8_t* base, int B, int Li, int Lt, int E) {
     float* cat_scale = cv.take<float>(f->fp8 >= 2 ? (int64_t)B * L : 0);
     float* row_stats = cv.take<float>((int64_t)B * L * (H / 64) * 2);
     uint16_t* lora_t = cv.take<uint16_t>(f->lora_rmax ? std::max<int64_t>((int64_t)B * L, EB) * f->lora_rmax : 0);
+    const int64_t fbc_n = f->fbc_threshold > 0.f ? (int64_t)B * Li * H : 0;
+    uint16_t* fbc_b0 = cv.take<uint16_t>(fbc_n);
+    uint16_t* fbc_b1 = cv.take<uint16_t>(fbc_n);
+    float* fbc_R = cv.take<float>(fbc_n);
+    float2* fbc_part = cv.take<float2>(fbc_n ? kFbcMaxBlocks : 0);
+    float* fbc_res = cv.take<float>(fbc_n ? 4 : 0);
     // sequence-parallel: qkv [W*L, 3H/W] and cat [L, H+mlp] are the caller's peer-mapped allocations (same sizes)
     const bool sp = f->sp_world > 1;
     uint16_t* qkv = sp ? static_cast<uint16_t*>(f->sp_qkv[f->sp_rank]) : cv.take<uint16_t>((int64_t)B * L * 3 * H);
@@ -100,6 +121,7 @@ int64_t carve(vcb_flux* f, uint8_t* base, int B, int Li, int Lt, int E) {
         f->e_guid = e_guid; f->e_vec = e_vec; f->vec = vec; f->svec = svec; f->mod_dbl = md; f->mod_sgl = ms;
         f->mod_final = mod_final; f->x = x; f->xm = xm; f->qkv = qkv; f->cat = cat; f->xm8 = xm8; f->row_scale = row_scale; f->row_stats = row_stats;
         f->cat8 = cat8; f->cat_scale = cat_scale; f->lora_t = lora_t;
+        f->fbc_buf[0] = fbc_b0; f->fbc_buf[1] = fbc_b1; f->fbc_R = fbc_R; f->fbc_part = fbc_part; f->fbc_res = fbc_res;
     }
     return cv.off;
 }
@@ -216,6 +238,24 @@ extern "C" int vcb_flux_set_fp8(vcb_flux* f, int32_t level) {
     return 0;
 }
 
+extern "C" int vcb_flux_set_first_block_cache(vcb_flux* f, float threshold) {
+    if (!f) return set_error("flux_set_first_block_cache: null engine");
+    if (!std::isfinite(threshold) || threshold < 0.f) return set_error("flux_set_first_block_cache: threshold must be a finite number >= 0 (0 = off)");
+    if (threshold > 0.f) {
+        if (f->sp_world > 1) return set_error("flux_set_first_block_cache: the skip decision would have to agree across the sequence-parallel ranks");
+        if (f->cfg.depth < 1) return set_error("flux_set_first_block_cache: the cache decides after the first double block (depth >= 1)");
+    }
+    if ((threshold > 0.f) != (f->fbc_threshold > 0.f)) f->prepared = false;    // the workspace layout depends on it
+    f->fbc_threshold = threshold;
+    return 0;
+}
+
+extern "C" int vcb_flux_cache_stats(const vcb_flux* f, int32_t* computed, int32_t* skipped, float* last_diff) {
+    if (!f || !computed || !skipped || !last_diff) return set_error("flux_cache_stats: null argument");
+    *computed = f->fbc_computed; *skipped = f->fbc_skipped; *last_diff = f->fbc_last_diff;
+    return 0;
+}
+
 extern "C" int vcb_flux_use_score_bounds(vcb_flux* f, int32_t enable) {
     if (!f) return set_error("flux_use_score_bounds: null engine");
     f->use_score_bounds = enable != 0;
@@ -248,6 +288,7 @@ extern "C" int vcb_flux_sp_attach(vcb_flux* f, int32_t world, int32_t rank, void
     if (f->cfg.heads % world) return set_error("flux_sp_attach: heads (%d) must be a multiple of world (%d)", f->cfg.heads, world);
     if (f->fp8) return set_error("flux_sp_attach: the sequence-parallel mode runs bf16 projections (switch vcb_flux_set_fp8 off first)");
     if (f->lora_rmax) return set_error("flux_sp_attach: the sequence-parallel mode takes merged LoRA weights only");
+    if (f->fbc_threshold > 0.f) return set_error("flux_sp_attach: the first-block cache decides per batch on one device (switch it off first)");
     for (int r = 0; r < world; ++r) {
         if (!qkv[r] || !cat[r] || !flags[r]) return set_error("flux_sp_attach: null buffer for rank %d", r);
         f->sp_qkv[r] = qkv[r]; f->sp_cat[r] = cat[r]; f->sp_flags[r] = flags[r];
@@ -271,6 +312,11 @@ extern "C" int vcb_flux_prepare(vcb_flux* f, void* workspace, int64_t workspace_
     carve(f, static_cast<uint8_t*>(workspace), B, Li, Lt, n_evals);
     f->B = B; f->Li = Li; f->Lt = Lt; f->L = Li + Lt; f->E = n_evals; f->seqlens = seqlens;
     f->prepared = false;
+    f->fbc_ref = 0; f->fbc_computed = 0; f->fbc_skipped = 0; f->fbc_last_diff = NAN;
+    if (f->fbc_threshold > 0.f && !f->fbc_host) {       // where vcb_flux_forward reads the cache's decision
+        cudaError_t e = cudaMallocHost(reinterpret_cast<void**>(&f->fbc_host), 4 * sizeof(float));
+        if (e != cudaSuccess) { f->fbc_host = nullptr; return set_error("flux_prepare: pinned memory: %s", cudaGetErrorString(e)); }
+    }
     const int H = c.hidden, EB = n_evals * B;
     int rc;
     // RoPE table (constant across steps; the reference recomputes it per call, model.py:110-111)
@@ -437,6 +483,37 @@ int double_ln(const vcb_flux* f, const StreamView* const sv[2], const uint16_t* 
     return vcb_ln_modulate_grouped(&a[0], &a[1], H, H, 6 * H, H, f->L, stream);
 }
 
+FbcRows fbc_rows(const vcb_flux* f) { return FbcRows{f->B, f->Li, f->Lt, f->L, f->cfg.hidden, f->seqlens}; }
+
+// First-block cache, right after double block 0: decide (one stream wait, except on the first evaluation since prepare, which is
+// always computed), then either write x = bf16(x1 + R) (skip) or make r_k the new r_ref and keep x1 for the residual R.
+int fbc_after_first_block(vcb_flux* f, cudaStream_t st, bool* skip) {
+    const bool first = f->fbc_computed == 0 && f->fbc_skipped == 0;
+    const FbcRows g = fbc_rows(f);
+    uint16_t* x0_rk = f->fbc_buf[f->fbc_ref ^ 1];
+    if (int rc = fbc_decide(x0_rk, f->x, f->fbc_buf[f->fbc_ref], g, first, f->fbc_threshold, f->fbc_part, f->fbc_res, st)) return rc;
+    *skip = false;
+    f->fbc_last_diff = INFINITY;
+    if (!first) {
+        cudaError_t e = cudaMemcpyAsync(f->fbc_host, f->fbc_res, 4 * sizeof(float), cudaMemcpyDeviceToHost, st);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+        if (e != cudaSuccess) return set_error("flux_forward: first-block cache decision: %s", cudaGetErrorString(e));
+        *skip = f->fbc_host[3] != 0.f;
+        f->fbc_last_diff = f->fbc_host[2];
+    }
+    if (*skip) {
+        ++f->fbc_skipped;
+        return fbc_apply_residual(f->x, f->fbc_R, g, st);
+    }
+    ++f->fbc_computed;
+    f->fbc_ref ^= 1;                                   // r_k is the reference of the next decisions
+    const int64_t H = f->cfg.hidden;
+    cudaError_t e = cudaMemcpy2DAsync(f->fbc_buf[f->fbc_ref ^ 1], (size_t)f->Li * H * 2, f->x + (int64_t)f->Lt * H, (size_t)f->L * H * 2,
+                                      (size_t)f->Li * H * 2, f->B, cudaMemcpyDeviceToDevice, st);
+    if (e != cudaSuccess) return set_error("flux_forward: first-block cache x1 copy: %s", cudaGetErrorString(e));
+    return 0;
+}
+
 }  // namespace
 
 extern "C" int vcb_flux_forward(vcb_flux* f, int32_t e, const void* img, int64_t ld_img, void* out, int64_t ld_out,
@@ -467,6 +544,13 @@ extern "C" int vcb_flux_forward(vcb_flux* f, int32_t e, const void* img, int64_t
         if (ce != cudaSuccess) return set_error("flux_forward: txt copy: %s", cudaGetErrorString(ce));
     }
     f->stats_valid = false;                  // x was just (re)written by img_in and the txt copy: no statistics yet
+    const bool fbc = f->fbc_threshold > 0.f;
+    bool skip = false;
+    if (fbc) {                               // x0: the img rows as img_in left them
+        cudaError_t ce = cudaMemcpy2DAsync(f->fbc_buf[f->fbc_ref ^ 1], (size_t)Li * H * 2, f->x + (int64_t)Lt * H, (size_t)L * H * 2,
+                                           (size_t)Li * H * 2, B, cudaMemcpyDeviceToDevice, st);
+        if (ce != cudaSuccess) return set_error("flux_forward: first-block cache x0 copy: %s", cudaGetErrorString(ce));
+    }
     const int64_t erow = (int64_t)e * B;     // first modulation row of this evaluation
     // ---- double-stream blocks (layers.py:158-196) ----
     for (int i = 0; i < c.depth; ++i) {
@@ -514,9 +598,13 @@ extern "C" int vcb_flux_forward(vcb_flux* f, int32_t e, const void* img, int64_t
             if ((rc = gemm_linear(f, g, lw, 2, stream))) return rc;
             f->stats_valid = true;
         }
+        if (i == 0 && fbc) {
+            if ((rc = fbc_after_first_block(f, st, &skip))) return rc;
+            if (skip) break;
+        }
     }
     // ---- single-stream blocks on the joint sequence (layers.py:232-245) ----
-    for (int i = 0; i < c.depth_single; ++i) {
+    for (int i = 0; !skip && i < c.depth_single; ++i) {
         const vcb_single_w& w = f->sgl[i];
         const uint16_t* mod = f->mod_sgl[i] + erow * 3 * H;
         if ((rc = stream_ln(f, s_all, mod + 0, mod + H, 3 * H, stream, f->fp8))) return rc;
@@ -527,6 +615,12 @@ extern "C" int vcb_flux_forward(vcb_flux* f, int32_t e, const void* img, int64_t
         if ((rc = stream_gemm(f, s_all, f->cat, ldc, 0, H + mlp, w.linear2, H, VCB_EPI_GATE_RES, f->x, H, 0, mod + 2 * H, 3 * H,
                               nullptr, nullptr, nullptr, nullptr, 0, 0, stream))) return rc;
         f->stats_valid = true;
+    }
+    if (fbc) {
+        if (!skip && (rc = fbc_store_residual(f->x, f->fbc_buf[f->fbc_ref ^ 1], f->fbc_R, fbc_rows(f), st))) return rc;
+        // the final LayerNorm computes its own statistics whenever the cache is on: a skipped evaluation (whose x no GEMM
+        // epilogue wrote) and a computed one then share the arithmetic, so equal residual streams give equal outputs
+        f->stats_valid = false;
     }
     // ---- final layer on the img rows (layers.py:255-259; chunk order shift, scale) ----
     {

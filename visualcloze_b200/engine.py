@@ -20,6 +20,18 @@ from ._lib import DoubleW, FluxConfigC, FluxWeightsC, LinearW, SingleW, StreamW,
 BF16 = torch.bfloat16
 
 
+def first_block_cache_threshold(threshold) -> float:
+    """Validated threshold of the first-block cache: None or 0 = off, else a finite number > 0."""
+    if threshold is None:
+        return 0.0
+    if isinstance(threshold, bool) or not isinstance(threshold, (int, float)):
+        raise ValueError(f"first-block cache threshold must be a number or None, got {threshold!r}")
+    t = float(threshold)
+    if not math.isfinite(t) or t < 0:
+        raise ValueError(f"first-block cache threshold must be finite and >= 0 (0 or None = off), got {threshold!r}")
+    return t
+
+
 def _freqs() -> Tensor:
     """frequency table of timestep_embedding (layers.py:39), computed exactly like the reference does."""
     half = 128
@@ -53,6 +65,7 @@ class FluxEngine:
         self._ws = workspace
         self._shape = None
         self._sp = None
+        self._fbc = 0.0
         self._freqs = _freqs().to(self.device)
 
     # ---- single-image sequence parallelism (SURVEY.md 8f-2) -------------------------------------------
@@ -61,6 +74,8 @@ class FluxEngine:
         ``prepare`` (identical on all ranks) and its LOCAL img rows (``sp.shard``) to ``forward``."""
         if sp is not None and sp.world > 1 and self.lora_mode == "unmerged":
             raise ValueError("sequence-parallel mode takes merged LoRA weights only")
+        if sp is not None and sp.world > 1 and self._fbc > 0:
+            raise ValueError("the first-block cache decides per batch on one GPU; switch it off before sequence parallelism")
         if sp is not None and self.params.num_heads % sp.world:
             raise ValueError(f"num_heads ({self.params.num_heads}) must be a multiple of the sequence-parallel world size ({sp.world})")
         if sp is None and self._sp is not None:
@@ -68,6 +83,26 @@ class FluxEngine:
             self._sp.release()
         self._sp = sp if (sp is not None and sp.world > 1) else None
         self._shape = None
+
+    # ---- first-block cache (vcb_flux_set_first_block_cache) ------------------------------------------
+    def set_first_block_cache(self, threshold) -> None:
+        """``threshold`` > 0: an evaluation whose double-block-0 residual moved by less than ``threshold`` (relative L1) since the
+        last computed evaluation reuses that evaluation's residual of the remaining blocks; 0 / None: off.  Each ``forward`` then
+        waits for its decision on the host (not capturable in a CUDA graph)."""
+        t = first_block_cache_threshold(threshold)
+        if t > 0 and self._sp is not None:
+            raise ValueError("the first-block cache decides per batch on one GPU; it is refused with sequence parallelism")
+        check(self.lib.vcb_flux_set_first_block_cache(self._h, t), "vcb_flux_set_first_block_cache")
+        if (t > 0) != (self._fbc > 0):
+            self._shape = None                 # the workspace layout changed: prepare again
+        self._fbc = t
+
+    def cache_stats(self) -> dict:
+        """{"computed", "skipped"}: evaluations since the last ``prepare``; "last_diff": the latest evaluation's relative change of
+        the first-block residual (inf for the first after ``prepare``, NaN before any)."""
+        c, s, d = C.c_int32(), C.c_int32(), C.c_float()
+        check(self.lib.vcb_flux_cache_stats(self._h, C.byref(c), C.byref(s), C.byref(d)), "vcb_flux_cache_stats")
+        return {"computed": int(c.value), "skipped": int(s.value), "last_diff": float(d.value)}
 
     # ---- weight packing -----------------------------------------------------------------------
     def _linear(self, name: str, fp8: bool = False) -> LinearW:

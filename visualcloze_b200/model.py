@@ -26,7 +26,7 @@ from dataclasses import dataclass, field
 import torch
 from torch import Tensor, nn
 
-from .engine import FluxEngine
+from .engine import FluxEngine, first_block_cache_threshold
 
 BF16 = torch.bfloat16
 
@@ -128,6 +128,7 @@ class Flux(nn.Module):
         self.linear_precision = "bf16"
         self.lora_mode = "merged"
         self._sp = None
+        self._fbc = 0.0
         kw = dict(device=device, dtype=dtype)
         for name, fin, fout in linear_table(params):
             _attach(self, name + ".weight", nn.Parameter(torch.empty(fout, fin, **kw), requires_grad=False))
@@ -193,6 +194,8 @@ class Flux(nn.Module):
             self._packed_key = key
             if getattr(self, "_sp", None) is not None:
                 self._engine.enable_sequence_parallel(self._sp)
+            if self._fbc:
+                self._engine.set_first_block_cache(self._fbc)
         return self._engine
 
     def set_linear_precision(self, precision: str) -> None:
@@ -229,9 +232,32 @@ class Flux(nn.Module):
         passes the same full inputs and receives the same full output.  Needs merged LoRA weights."""
         if sp is not None and sp.world > 1 and self.lora_mode == "unmerged":
             raise ValueError("sequence-parallel mode takes merged LoRA weights only (set_lora_mode('merged') first)")
+        if sp is not None and sp.world > 1 and self._fbc:
+            raise ValueError("the first-block cache decides per batch on one GPU (enable_first_block_cache(None) first)")
         self._sp = sp
         if self._engine is not None:
             self._engine.enable_sequence_parallel(sp)
+
+    def enable_first_block_cache(self, threshold: float | None) -> None:
+        """Opt-in first-block cache (FBCache; no counterpart in the reference, NOT the reference's numerics).  Within one sampler
+        solve, every evaluation runs double block 0; when its img-row residual differs from the one of the last fully computed
+        evaluation by less than ``threshold`` (sum|r - r_ref| / sum|r_ref| over the valid rows of the whole batch), the other blocks
+        are skipped and their residual from that evaluation is reused.  The first evaluation of a solve is always computed.
+        ``None`` or 0 switches it off (the default).  Composes with both LoRA modes and the fp8 precisions; refused with sequence
+        parallelism.  No threshold is recommended: quality on trained weights has not been measured (DESIGN.md §2d)."""
+        t = first_block_cache_threshold(threshold)
+        if t > 0 and self._sp is not None and self._sp.world > 1:
+            raise ValueError("the first-block cache decides per batch on one GPU; it is refused with sequence parallelism")
+        self._fbc = t
+        if self._engine is not None:
+            self._engine.set_first_block_cache(t)
+
+    def cache_stats(self) -> dict:
+        """First-block cache counters of the latest solve (or ``forward``): evaluations "computed" and "skipped" and the latest
+        "last_diff" (inf for the first evaluation of a solve, NaN before any)."""
+        if self._engine is None:
+            return {"computed": 0, "skipped": 0, "last_diff": math.nan}
+        return self._engine.cache_stats()
 
     # ------------------------------------------------------------------------------------------
     def forward(self, img: Tensor, img_ids: Tensor, txt: Tensor, txt_ids: Tensor, timesteps: Tensor, y: Tensor,

@@ -111,7 +111,8 @@ def _expand_state_dict(model, sd: dict) -> dict:
 class VisualClozeModel:
     def __init__(self, model_path=None, model_name="flux-dev-fill-lora", max_length=512, lora_rank=256, atol=1e-6, rtol=1e-3,
                  solver="euler", time_shifting_factor=1, resolution=384, precision="bf16", *, model=None, ae_decoder=None,
-                 ae_encoder=None, t5=None, clip=None, encode=None, device=None, flux_ckpt=None, ae_ckpt=None, lora_mode="merged"):
+                 ae_encoder=None, t5=None, clip=None, encode=None, device=None, flux_ckpt=None, ae_ckpt=None, lora_mode="merged",
+                 first_block_cache=None):
         """Positional arguments as the reference (visualcloze.py:79-82).  The reference constructor also pulls the base
         FLUX.1-Fill-dev weights (``load_flow_model``: ``$FLUX_DEV_FILL`` or a hub download) and the FLUX VAE
         (``AutoencoderKL.from_pretrained``); there is no network on the inference box, so here they come from files:
@@ -119,7 +120,9 @@ class VisualClozeModel:
         ``ae.safetensors`` or diffusers ``vae/diffusion_pytorch_model.safetensors`` -- keys are converted).  Pre-built
         ``model`` / ``ae_decoder`` / ``ae_encoder`` objects are used as they are.  Nothing is ever run on never-loaded
         parameters: the engines refuse to pack them.  ``lora_mode``: "merged" (default) or "unmerged", set on the flow model
-        built or given (``FluxLoraWrapper.set_lora_mode``)."""
+        built or given (``FluxLoraWrapper.set_lora_mode``).  ``first_block_cache``: None (default, off) or the threshold of the
+        opt-in first-block cache (``Flux.enable_first_block_cache``), set on the flow model likewise; the grid solve and the
+        SDEdit solve each start it afresh."""
         if precision != "bf16":
             raise NotImplementedError("the sm_90a kernels implement the reference's default bf16 path only")
         if model_name != "flux-dev-fill-lora":
@@ -143,6 +146,7 @@ class VisualClozeModel:
                                      f"e.g. {res.unexpected_keys[:3]}")
                 del sd
         model.set_lora_mode(lora_mode)
+        model.enable_first_block_cache(first_block_cache)
         self.model = model
         if model_path is not None:
             ckpt = _load_file(model_path, self.device)
