@@ -169,7 +169,9 @@ int vcb_attention_fwd_ex(const vcb_attn_args* args, void* stream);
 int vcb_debug_attn4_timeline(unsigned long long* out, int32_t capacity);
 
 /* ---- AdaLN modulated LayerNorm (layers.py:163-164,191,195,234,257):
- *      y = bf16( bf16(1 + scale[b]) * LayerNorm(x) + shift[b] ), eps 1e-6, no affine; hidden % 256 == 0.
+ *      y = bf16( bf16(1 + scale[b]) * LayerNorm(x) + shift[b] ), eps 1e-6, no affine.
+ *      Every vcb_ln_modulate* entry point needs hidden % 256 == 0 and hidden <= 6144 (the modulation vectors of a block are
+ *      staged in 8 * hidden bytes of shared memory).
  *      Logical row r = (b, i) with b = r / rows_per_batch lives at physical row b * batch_rows + i of x and y
  *      (batch_rows = 0 means rows_per_batch, i.e. a plain [rows, hidden] matrix). */
 int vcb_ln_modulate(const void* x, int64_t ldx, void* y, int64_t ldy, const void* shift, const void* scale,
@@ -177,7 +179,7 @@ int vcb_ln_modulate(const void* x, int64_t ldx, void* y, int64_t ldy, const void
                     void* stream);
 
 /* Two row ranges of the same [*, hidden] buffers with their own modulation vectors in ONE launch (the img and txt streams of
- * a DoubleStreamBlock): ldx / ldy / mod_stride / hidden / batch_rows are shared. */
+ * a DoubleStreamBlock): ldx / ldy / mod_stride / hidden / batch_rows (> 0) are shared.  a1 may be NULL: one problem. */
 typedef struct vcb_ln_args { const void* x; void* y; const void* shift; const void* scale; int32_t rows, rows_per_batch; } vcb_ln_args;
 int vcb_ln_modulate_grouped(const vcb_ln_args* a0, const vcb_ln_args* a1, int64_t ldx, int64_t ldy, int64_t mod_stride,
                             int32_t hidden, int32_t batch_rows, void* stream);

@@ -601,34 +601,37 @@ extern "C" int vcb_sp_barrier(int32_t* const* flags, int32_t world, int32_t rank
 // elementwise
 // ------------------------------------------------------------------------------------------------
 namespace {
-int ln_launch(const vcb_ln_args* a0, const vcb_ln_args* a1, int64_t ldx, int64_t ldy, int64_t mod_stride, int32_t hidden,
-              int32_t batch_rows, void* stream) {
-    if (hidden % 256 || hidden > 256 * kLnMaxChunks) return set_error("ln_modulate: hidden must be a multiple of 256, <= %d", 256 * kLnMaxChunks);
-    if (ldx % 8 || ldy % 8 || mod_stride % 8) return set_error("ln_modulate: strides must be multiples of 8");
-    LnProblem p[2] = {};
+// One AdaLN LayerNorm launch (elementwise.cuh) for the five entry points below: one or two problems (a1 may be NULL), e4m3
+// output with per-row scales when fp8, statistics from the producing GEMM when with_stats.  `fn` prefixes the error messages.
+int ln_launch(const char* fn, const vcb_ln_args* a0, const vcb_ln_args* a1, bool fp8, float* row_scale0, float* row_scale1,
+              bool with_stats, const void* stats0, const void* stats1, int32_t n_slots, int64_t ldx, int64_t ldy, int64_t mod_stride,
+              int32_t hidden, int32_t batch_rows, void* stream) {
+    if (!a0) return set_error("%s: null problem", fn);
+    if (hidden % 256 || hidden > kLnMaxHidden) return set_error("%s: hidden must be a multiple of 256, <= %d", fn, kLnMaxHidden);
+    if (ldx % 8 || mod_stride % 8 || ldy % (fp8 ? 16 : 8))
+        return set_error("%s: ldx / mod_stride must be multiples of 8, the output stride of %d", fn, fp8 ? 16 : 8);
+    if (with_stats && n_slots <= 0) return set_error("%s: n_slots must be positive", fn);
     const vcb_ln_args* a[2] = {a0, a1};
+    float* rs[2] = {row_scale0, row_scale1};
+    const void* st[2] = {stats0, stats1};
+    LnProblem p[2] = {};
     for (int i = 0; i < 2; ++i) {
         if (!a[i]) continue;
         if (!a[i]->x || !a[i]->y || !a[i]->shift || !a[i]->scale || a[i]->rows <= 0 || a[i]->rows_per_batch <= 0)
-            return set_error("ln_modulate: bad arguments");
-        p[i] = LnProblem{(const __nv_bfloat16*)a[i]->x, (__nv_bfloat16*)a[i]->y, (const __nv_bfloat16*)a[i]->shift,
+            return set_error("%s: bad arguments", fn);
+        if (fp8 && !rs[i]) return set_error("%s: null row_scale", fn);
+        if (with_stats && !st[i]) return set_error("%s: null stats", fn);
+        p[i] = LnProblem{(const __nv_bfloat16*)a[i]->x, a[i]->y, rs[i], (const float2*)st[i], (const __nv_bfloat16*)a[i]->shift,
                          (const __nv_bfloat16*)a[i]->scale, a[i]->rows, a[i]->rows_per_batch, (a[i]->rows + kLnWarps - 1) / kLnWarps};
     }
+    if (batch_rows <= 0) return set_error("%s: batch_rows (rows of one sample in the joint buffer) is required", fn);
     if (int rc = ensure_device()) return rc;
     ProfScope prof(PROF_LN, stream);
-    const int br = batch_rows > 0 ? batch_rows : p[0].rows_per_batch;
-    const dim3 grid(p[0].blocks + p[1].blocks), block(kLnWarps * 32);
-    // VCB_LN_ONEPASS=1: the round-1 kernel (row held in registers, 3 blocks per SM) for A/B; default = two-pass, 6 blocks per SM
-    static const bool onepass = [] { const char* e = getenv("VCB_LN_ONEPASS"); return e && atoi(e); }();
-    cudaError_t e = !onepass
-        ? launch_pdl(ln_modulate2_kernel, grid, block, (size_t)hidden * 8, (cudaStream_t)stream, 1, p[0], p[1], (long long)ldx,
-                     (long long)ldy, (long long)mod_stride, (int)hidden, br)
-        : hidden <= 12 * 256
-        ? launch_pdl(ln_modulate_kernel<12, 3>, grid, block, (size_t)hidden * 4, (cudaStream_t)stream, 1, p[0], p[1], (long long)ldx,
-                     (long long)ldy, (long long)mod_stride, (int)hidden, br)
-        : launch_pdl(ln_modulate_kernel<kLnMaxChunks, 2>, grid, block, (size_t)hidden * 4, (cudaStream_t)stream, 1, p[0], p[1], (long long)ldx,
-                     (long long)ldy, (long long)mod_stride, (int)hidden, br);
-    if (e != cudaSuccess) return set_error("ln_modulate launch: %s", cudaGetErrorString(e));
+    auto kern = fp8 ? (with_stats ? ln_modulate_fp8_stats_kernel : ln_modulate_fp8_kernel)
+                    : (with_stats ? ln_modulate_stats_kernel : ln_modulate2_kernel);
+    cudaError_t e = launch_pdl(kern, dim3(p[0].blocks + p[1].blocks), dim3(kLnWarps * 32), (size_t)hidden * 8, (cudaStream_t)stream, 1,
+                               p[0], p[1], (long long)ldx, (long long)ldy, (long long)mod_stride, (int)hidden, (int)batch_rows, (int)n_slots);
+    if (e != cudaSuccess) return set_error("%s launch: %s", fn, cudaGetErrorString(e));
     count_launch();
     return 0;
 }
@@ -638,70 +641,33 @@ extern "C" int vcb_ln_modulate(const void* x, int64_t ldx, void* y, int64_t ldy,
                                int64_t mod_stride, int32_t rows, int32_t hidden, int32_t rows_per_batch, int32_t batch_rows,
                                void* stream) {
     const vcb_ln_args a{x, y, shift, scale, rows, rows_per_batch};
-    return ln_launch(&a, nullptr, ldx, ldy, mod_stride, hidden, batch_rows, stream);
+    return ln_launch("ln_modulate", &a, nullptr, false, nullptr, nullptr, false, nullptr, nullptr, 0, ldx, ldy, mod_stride, hidden,
+                     batch_rows > 0 ? batch_rows : rows_per_batch, stream);
 }
 
 extern "C" int vcb_ln_modulate_grouped(const vcb_ln_args* a0, const vcb_ln_args* a1, int64_t ldx, int64_t ldy, int64_t mod_stride,
                                        int32_t hidden, int32_t batch_rows, void* stream) {
-    if (!a0 || !a1) return set_error("ln_modulate (grouped): null problem");
-    if (batch_rows <= 0) return set_error("ln_modulate (grouped): batch_rows (rows of one sample in the joint buffer) is required");
-    return ln_launch(a0, a1, ldx, ldy, mod_stride, hidden, batch_rows, stream);
+    return ln_launch("ln_modulate_grouped", a0, a1, false, nullptr, nullptr, false, nullptr, nullptr, 0, ldx, ldy, mod_stride, hidden,
+                     batch_rows, stream);
 }
 
 extern "C" int vcb_ln_modulate_stats(const vcb_ln_args* a0, const vcb_ln_args* a1, const void* stats0, const void* stats1, int32_t n_slots,
                                      int64_t ldx, int64_t ldy, int64_t mod_stride, int32_t hidden, int32_t batch_rows, void* stream) {
-    if (!a0 || !stats0 || (a1 && !stats1) || n_slots <= 0) return set_error("ln_modulate_stats: null problem / stats");
-    if (hidden % 256) return set_error("ln_modulate_stats: hidden must be a multiple of 256");
-    if (ldx % 8 || ldy % 8 || mod_stride % 8) return set_error("ln_modulate_stats: strides must be multiples of 8");
-    if (batch_rows <= 0) return set_error("ln_modulate_stats: batch_rows (rows of one sample in the joint buffer) is required");
-    LnStatsProblem p[2] = {};
-    const vcb_ln_args* a[2] = {a0, a1};
-    const void* st[2] = {stats0, stats1};
-    for (int i = 0; i < 2; ++i) {
-        if (!a[i]) continue;
-        if (!a[i]->x || !a[i]->y || !a[i]->shift || !a[i]->scale || a[i]->rows <= 0 || a[i]->rows_per_batch <= 0)
-            return set_error("ln_modulate_stats: bad arguments");
-        p[i] = LnStatsProblem{(const __nv_bfloat16*)a[i]->x, (__nv_bfloat16*)a[i]->y, (const __nv_bfloat16*)a[i]->shift,
-                              (const __nv_bfloat16*)a[i]->scale, (const float2*)st[i], a[i]->rows, a[i]->rows_per_batch,
-                              (a[i]->rows + kLnWarps - 1) / kLnWarps};
-    }
-    if (int rc = ensure_device()) return rc;
-    ProfScope prof(PROF_LN, stream);
-    const dim3 grid(p[0].blocks + p[1].blocks), block(kLnWarps * 32);
-    cudaError_t e = launch_pdl(ln_modulate_stats_kernel, grid, block, (size_t)hidden * 8, (cudaStream_t)stream, 1, p[0], p[1], (long long)ldx,
-                               (long long)ldy, (long long)mod_stride, (int)hidden, (int)batch_rows, (int)n_slots);
-    if (e != cudaSuccess) return set_error("ln_modulate_stats launch: %s", cudaGetErrorString(e));
-    count_launch();
-    return 0;
+    return ln_launch("ln_modulate_stats", a0, a1, false, nullptr, nullptr, true, stats0, stats1, n_slots, ldx, ldy, mod_stride, hidden,
+                     batch_rows, stream);
 }
 
 extern "C" int vcb_ln_modulate_fp8(const vcb_ln_args* a0, const vcb_ln_args* a1, float* row_scale0, float* row_scale1, int64_t ldx,
                                    int64_t ld8, int64_t mod_stride, int32_t hidden, int32_t batch_rows, void* stream) {
-    if (!a0 || !row_scale0 || (a1 && !row_scale1)) return set_error("ln_modulate_fp8: null problem / row_scale");
-    if (hidden % 256 || hidden > 256 * kLnMaxChunks) return set_error("ln_modulate_fp8: hidden must be a multiple of 256, <= %d", 256 * kLnMaxChunks);
-    if (ldx % 8 || ld8 % 16 || mod_stride % 8) return set_error("ln_modulate_fp8: ldx / mod_stride must be multiples of 8, ld8 of 16");
-    if (batch_rows <= 0) return set_error("ln_modulate_fp8: batch_rows (rows of one sample in the joint buffer) is required");
-    LnFp8Problem p[2] = {};
-    const vcb_ln_args* a[2] = {a0, a1};
-    float* rs[2] = {row_scale0, row_scale1};
-    for (int i = 0; i < 2; ++i) {
-        if (!a[i]) continue;
-        if (!a[i]->x || !a[i]->y || !a[i]->shift || !a[i]->scale || a[i]->rows <= 0 || a[i]->rows_per_batch <= 0)
-            return set_error("ln_modulate_fp8: bad arguments");
-        p[i] = LnFp8Problem{(const __nv_bfloat16*)a[i]->x, (uint8_t*)a[i]->y, rs[i], (const __nv_bfloat16*)a[i]->shift,
-                            (const __nv_bfloat16*)a[i]->scale, a[i]->rows, a[i]->rows_per_batch, (a[i]->rows + kLnWarps - 1) / kLnWarps};
-    }
-    if (int rc = ensure_device()) return rc;
-    ProfScope prof(PROF_LN, stream);
-    const dim3 grid(p[0].blocks + p[1].blocks), block(kLnWarps * 32);
-    cudaError_t e = hidden <= 12 * 256
-        ? launch_pdl(ln_modulate_fp8_kernel<12>, grid, block, (size_t)hidden * 4, (cudaStream_t)stream, 1, p[0], p[1], (long long)ldx,
-                     (long long)ld8, (long long)mod_stride, (int)hidden, (int)batch_rows)
-        : launch_pdl(ln_modulate_fp8_kernel<kLnMaxChunks>, grid, block, (size_t)hidden * 4, (cudaStream_t)stream, 1, p[0], p[1], (long long)ldx,
-                     (long long)ld8, (long long)mod_stride, (int)hidden, (int)batch_rows);
-    if (e != cudaSuccess) return set_error("ln_modulate_fp8 launch: %s", cudaGetErrorString(e));
-    count_launch();
-    return 0;
+    return ln_launch("ln_modulate_fp8", a0, a1, true, row_scale0, row_scale1, false, nullptr, nullptr, 0, ldx, ld8, mod_stride, hidden,
+                     batch_rows, stream);
+}
+
+extern "C" int vcb_ln_modulate_fp8_stats(const vcb_ln_args* a0, const vcb_ln_args* a1, float* row_scale0, float* row_scale1, const void* stats0,
+                                         const void* stats1, int32_t n_slots, int64_t ldx, int64_t ld8, int64_t mod_stride, int32_t hidden,
+                                         int32_t batch_rows, void* stream) {
+    return ln_launch("ln_modulate_fp8_stats", a0, a1, true, row_scale0, row_scale1, true, stats0, stats1, n_slots, ldx, ld8, mod_stride,
+                     hidden, batch_rows, stream);
 }
 
 extern "C" int vcb_quantize_rows_e4m3(const void* x, int64_t ldx, void* y8, int64_t ld8, float* row_scale, int64_t rows, int32_t K,
@@ -716,33 +682,6 @@ extern "C" int vcb_quantize_rows_e4m3(const void* x, int64_t ldx, void* y8, int6
     cudaError_t e = launch_pdl(quantize_rows_e4m3_kernel, dim3((unsigned)rows), dim3(kQuantThreads), (size_t)0, (cudaStream_t)stream, 1,
                                (const __nv_bfloat16*)x, (long long)ldx, (uint8_t*)y8, (long long)ld8, row_scale, (int)K);
     if (e != cudaSuccess) return set_error("quantize_rows_e4m3 launch: %s", cudaGetErrorString(e));
-    count_launch();
-    return 0;
-}
-
-extern "C" int vcb_ln_modulate_fp8_stats(const vcb_ln_args* a0, const vcb_ln_args* a1, float* row_scale0, float* row_scale1, const void* stats0,
-                                         const void* stats1, int32_t n_slots, int64_t ldx, int64_t ld8, int64_t mod_stride, int32_t hidden,
-                                         int32_t batch_rows, void* stream) {
-    if (!a0 || !row_scale0 || !stats0 || (a1 && (!row_scale1 || !stats1)) || n_slots <= 0) return set_error("ln_modulate_fp8_stats: null problem / row_scale / stats");
-    if (hidden % 256) return set_error("ln_modulate_fp8_stats: hidden must be a multiple of 256");
-    if (ldx % 8 || ld8 % 16 || mod_stride % 8) return set_error("ln_modulate_fp8_stats: ldx / mod_stride must be multiples of 8, ld8 of 16");
-    if (batch_rows <= 0) return set_error("ln_modulate_fp8_stats: batch_rows (rows of one sample in the joint buffer) is required");
-    LnFp8Problem p[2] = {};
-    const vcb_ln_args* a[2] = {a0, a1};
-    float* rs[2] = {row_scale0, row_scale1};
-    for (int i = 0; i < 2; ++i) {
-        if (!a[i]) continue;
-        if (!a[i]->x || !a[i]->y || !a[i]->shift || !a[i]->scale || a[i]->rows <= 0 || a[i]->rows_per_batch <= 0)
-            return set_error("ln_modulate_fp8_stats: bad arguments");
-        p[i] = LnFp8Problem{(const __nv_bfloat16*)a[i]->x, (uint8_t*)a[i]->y, rs[i], (const __nv_bfloat16*)a[i]->shift,
-                            (const __nv_bfloat16*)a[i]->scale, a[i]->rows, a[i]->rows_per_batch, (a[i]->rows + kLnWarps - 1) / kLnWarps};
-    }
-    if (int rc = ensure_device()) return rc;
-    ProfScope prof(PROF_LN, stream);
-    const dim3 grid(p[0].blocks + p[1].blocks), block(kLnWarps * 32);
-    cudaError_t e = launch_pdl(ln_modulate_fp8_stats_kernel, grid, block, (size_t)hidden * 8, (cudaStream_t)stream, 1, p[0], p[1], (const float2*)stats0,
-                               (const float2*)stats1, (int)n_slots, (long long)ldx, (long long)ld8, (long long)mod_stride, (int)hidden, (int)batch_rows);
-    if (e != cudaSuccess) return set_error("ln_modulate_fp8_stats launch: %s", cudaGetErrorString(e));
     count_launch();
     return 0;
 }

@@ -436,51 +436,30 @@ int stream_gemm(const vcb_flux* f, const StreamView& sv, const uint16_t* a_buf, 
     return gemm_linear(f, g, w, stream);
 }
 
-// fp8: the LayerNorm feeds an fp8 projection -> e4m3 rows + per-row scales instead of bf16 rows
-int stream_ln(const vcb_flux* f, const StreamView& sv, const uint16_t* shift, const uint16_t* scale, int64_t mod_stride,
-              void* stream, bool fp8 = false) {
-    const int H = f->cfg.hidden;
-    if (fp8) {
-        vcb_ln_args a{f->x + (int64_t)sv.off * H, f->xm8 + (int64_t)sv.off * H, shift, scale, f->B * sv.rows, sv.rows};
-        if (f->stats_valid)
-            return vcb_ln_modulate_fp8_stats(&a, nullptr, f->row_scale + sv.off, nullptr, f->row_stats + (int64_t)sv.off * (H / 64) * 2, nullptr,
-                                             H / 64, H, H, mod_stride, H, f->L, stream);
-        return vcb_ln_modulate_fp8(&a, nullptr, f->row_scale + sv.off, nullptr, H, H, mod_stride, H, f->L, stream);
+// The AdaLN LayerNorm of one stream, or of both streams of a DoubleStreamBlock in one launch (sv1 != nullptr).  shift0 / shift1:
+// the stream's shift vector; its scale follows at + hidden.
+// fp8: the LayerNorm feeds an fp8 projection -> e4m3 rows + per-row scales instead of bf16 rows.
+int adaln(const vcb_flux* f, const StreamView& sv0, const uint16_t* shift0, const StreamView* sv1, const uint16_t* shift1, int64_t mod_stride,
+          bool fp8, void* stream) {
+    const int H = f->cfg.hidden, ns = H / 64;
+    const StreamView* sv[2] = {&sv0, sv1};
+    const uint16_t* shift[2] = {shift0, shift1};
+    vcb_ln_args a[2] = {};
+    float* rs[2] = {};
+    const float* st[2] = {};
+    for (int s = 0; s < (sv1 ? 2 : 1); ++s) {
+        const int64_t off = sv[s]->off;
+        void* y = fp8 ? (void*)(f->xm8 + off * H) : (void*)(f->xm + off * H);
+        a[s] = vcb_ln_args{f->x + off * H, y, shift[s], shift[s] + H, f->B * sv[s]->rows, sv[s]->rows};
+        rs[s] = f->row_scale + off;
+        st[s] = f->row_stats + off * ns * 2;
     }
-    if (f->stats_valid) {
-        const int ns = H / 64;
-        vcb_ln_args a{f->x + (int64_t)sv.off * H, f->xm + (int64_t)sv.off * H, shift, scale, f->B * sv.rows, sv.rows};
-        return vcb_ln_modulate_stats(&a, nullptr, f->row_stats + (int64_t)sv.off * ns * 2, nullptr, ns, H, H, mod_stride, H, f->L, stream);
-    }
-    return vcb_ln_modulate(f->x + (int64_t)sv.off * H, H, f->xm + (int64_t)sv.off * H, H, shift, scale, mod_stride,
-                           f->B * sv.rows, H, sv.rows, f->L, stream);
-}
-
-// both streams of a DoubleStreamBlock in one LayerNorm launch; mod_col = column of `shift` in the 6H modulation row
-int double_ln(const vcb_flux* f, const StreamView* const sv[2], const uint16_t* const mod[2], int mod_col, void* stream) {
-    const int H = f->cfg.hidden;
-    vcb_ln_args a[2];
-    if (f->fp8) {
-        for (int s = 0; s < 2; ++s)
-            a[s] = vcb_ln_args{f->x + (int64_t)sv[s]->off * H, f->xm8 + (int64_t)sv[s]->off * H, mod[s] + mod_col, mod[s] + mod_col + H,
-                               f->B * sv[s]->rows, sv[s]->rows};
-        if (f->stats_valid) {
-            const int ns = H / 64;
-            return vcb_ln_modulate_fp8_stats(&a[0], &a[1], f->row_scale + sv[0]->off, f->row_scale + sv[1]->off,
-                                             f->row_stats + (int64_t)sv[0]->off * ns * 2, f->row_stats + (int64_t)sv[1]->off * ns * 2, ns, H, H,
-                                             6 * H, H, f->L, stream);
-        }
-        return vcb_ln_modulate_fp8(&a[0], &a[1], f->row_scale + sv[0]->off, f->row_scale + sv[1]->off, H, H, 6 * H, H, f->L, stream);
-    }
-    for (int s = 0; s < 2; ++s)
-        a[s] = vcb_ln_args{f->x + (int64_t)sv[s]->off * H, f->xm + (int64_t)sv[s]->off * H, mod[s] + mod_col, mod[s] + mod_col + H,
-                           f->B * sv[s]->rows, sv[s]->rows};
-    if (f->stats_valid) {
-        const int ns = H / 64;
-        return vcb_ln_modulate_stats(&a[0], &a[1], f->row_stats + (int64_t)sv[0]->off * ns * 2, f->row_stats + (int64_t)sv[1]->off * ns * 2, ns,
-                                     H, H, 6 * H, H, f->L, stream);
-    }
-    return vcb_ln_modulate_grouped(&a[0], &a[1], H, H, 6 * H, H, f->L, stream);
+    const vcb_ln_args* a1 = sv1 ? &a[1] : nullptr;
+    if (f->stats_valid)
+        return fp8 ? vcb_ln_modulate_fp8_stats(&a[0], a1, rs[0], rs[1], st[0], st[1], ns, H, H, mod_stride, H, f->L, stream)
+                   : vcb_ln_modulate_stats(&a[0], a1, st[0], st[1], ns, H, H, mod_stride, H, f->L, stream);
+    return fp8 ? vcb_ln_modulate_fp8(&a[0], a1, rs[0], rs[1], H, H, mod_stride, H, f->L, stream)
+               : vcb_ln_modulate_grouped(&a[0], a1, H, H, mod_stride, H, f->L, stream);
 }
 
 FbcRows fbc_rows(const vcb_flux* f) { return FbcRows{f->B, f->Li, f->Lt, f->L, f->cfg.hidden, f->seqlens}; }
@@ -559,7 +538,7 @@ extern "C" int vcb_flux_forward(vcb_flux* f, int32_t e, const void* img, int64_t
         const StreamView* sv[2] = {&s_img, &s_txt};
         const uint16_t* mod[2] = {f->mod_dbl[2 * i] + erow * 6 * H, f->mod_dbl[2 * i + 1] + erow * 6 * H};
         // both streams of a block share each launch (img first, txt fills the img problem's partial last wave)
-        if ((rc = double_ln(f, sv, mod, 0, stream))) return rc;
+        if ((rc = adaln(f, s_img, mod[0], &s_txt, mod[1], 6 * H, f->fp8, stream))) return rc;
         {
             vcb_gemm_args g[2];
             const vcb_linear_w* lw[2] = {&sw[0]->qkv, &sw[1]->qkv};
@@ -579,7 +558,7 @@ extern "C" int vcb_flux_forward(vcb_flux* f, int32_t e, const void* img, int64_t
             if ((rc = gemm_linear(f, g, lw, 2, stream))) return rc;
             f->stats_valid = true;             // both streams' rows of x now have their LayerNorm statistics in row_stats
         }
-        if ((rc = double_ln(f, sv, mod, 3 * H, stream))) return rc;
+        if ((rc = adaln(f, s_img, mod[0] + 3 * H, &s_txt, mod[1] + 3 * H, 6 * H, f->fp8, stream))) return rc;
         {
             vcb_gemm_args g[2];
             const vcb_linear_w* lw[2] = {&sw[0]->mlp0, &sw[1]->mlp0};
@@ -607,7 +586,7 @@ extern "C" int vcb_flux_forward(vcb_flux* f, int32_t e, const void* img, int64_t
     for (int i = 0; !skip && i < c.depth_single; ++i) {
         const vcb_single_w& w = f->sgl[i];
         const uint16_t* mod = f->mod_sgl[i] + erow * 3 * H;
-        if ((rc = stream_ln(f, s_all, mod + 0, mod + H, 3 * H, stream, f->fp8))) return rc;
+        if ((rc = adaln(f, s_all, mod, nullptr, nullptr, 3 * H, f->fp8, stream))) return rc;
         if ((rc = stream_gemm(f, s_all, f->xm, H, 0, H, w.linear1, 3 * H + mlp, VCB_EPI_LINEAR1, f->qkv, 3 * H, 0, nullptr, 0,
                               nullptr, w.q_scale, w.k_scale, f->cat, ldc, H, stream))) return rc;
         if ((rc = joint_attention(f, ldc, w.attn_score_bound, stream))) return rc;
@@ -625,7 +604,7 @@ extern "C" int vcb_flux_forward(vcb_flux* f, int32_t e, const void* img, int64_t
     // ---- final layer on the img rows (layers.py:255-259; chunk order shift, scale) ----
     {
         const uint16_t* mod = f->mod_final + erow * 2 * H;
-        if ((rc = stream_ln(f, s_img, mod + 0, mod + H, 2 * H, stream))) return rc;
+        if ((rc = adaln(f, s_img, mod, nullptr, nullptr, 2 * H, false, stream))) return rc;
         vcb_gemm_args g{};
         g.M = B * Li; g.N = c.out_channels; g.K = H;
         g.A = f->xm + (int64_t)Lt * H; g.lda = H; g.a_batch_stride = (int64_t)L * H;

@@ -162,31 +162,53 @@ def ln_modulate(x: torch.Tensor, shift: torch.Tensor, scale: torch.Tensor, out: 
     return out
 
 
-def ln_modulate_grouped(x: torch.Tensor, out: torch.Tensor, problems: list, hidden: int, batch_rows: int, mod_stride: int) -> None:
-    """Two row ranges of the joint buffers in one launch.  ``problems``: two tuples (row_offset, rows, rows_per_batch, shift, scale);
-    x / out are the [*, hidden] joint buffers (vcb_ln_modulate_grouped)."""
-    _req(x, BF16, "x"); _req(out, BF16, "out")
-    args = []
-    for off, rows, rpb, shift, scale in problems:
+def _ln_launch(x: torch.Tensor, out: torch.Tensor, problems: list, hidden: int, batch_rows: int, mod_stride: int,
+               row_scale: torch.Tensor | None = None, stats: torch.Tensor | None = None) -> None:
+    """One AdaLN LayerNorm launch over one or two problems (row_offset, rows, rows_per_batch, shift, scale) of the [*, hidden]
+    buffers x / out: out bf16, or float8_e4m3fn with ``row_scale`` [*] fp32; ``stats`` [*, n_slots, 2] fp32: row statistics
+    supplied by the producing GEMM.  row_scale and stats are indexed by the row of x, like out."""
+    fp8 = out.dtype == torch.float8_e4m3fn
+    _req(x, BF16, "x"); _req(out, torch.float8_e4m3fn if fp8 else BF16, "out")
+    if fp8:
+        _req(row_scale, torch.float32, "row_scale")
+    if stats is not None:
+        _req(stats, torch.float32, "stats")
+    args, rs, st = [None, None], [None, None], [None, None]
+    for i, (off, rows, rpb, shift, scale) in enumerate(problems):
         _req(shift, BF16, "shift"); _req(scale, BF16, "scale")
         a = _lib.LnArgs()
-        a.x, a.y = x.data_ptr() + off * x.stride(0) * 2, out.data_ptr() + off * out.stride(0) * 2
+        a.x, a.y = x.data_ptr() + off * x.stride(0) * 2, out.data_ptr() + off * out.stride(0) * out.element_size()
         a.shift, a.scale, a.rows, a.rows_per_batch = shift.data_ptr(), scale.data_ptr(), rows, rpb
-        args.append(a)
-    check(_lib.lib().vcb_ln_modulate_grouped(C.byref(args[0]), C.byref(args[1]), x.stride(0), out.stride(0), mod_stride, hidden,
-                                             batch_rows, _stream()), "vcb_ln_modulate_grouped")
+        args[i] = C.byref(a)
+        if fp8:
+            rs[i] = row_scale.data_ptr() + off * 4
+        if stats is not None:
+            st[i] = stats.data_ptr() + off * stats.stride(0) * 4
+    common = (x.stride(0), out.stride(0), mod_stride, hidden, batch_rows, _stream())
+    lib = _lib.lib()
+    if stats is not None and fp8:
+        check(lib.vcb_ln_modulate_fp8_stats(*args, *rs, *st, stats.shape[1], *common), "vcb_ln_modulate_fp8_stats")
+    elif stats is not None:
+        check(lib.vcb_ln_modulate_stats(*args, *st, stats.shape[1], *common), "vcb_ln_modulate_stats")
+    elif fp8:
+        check(lib.vcb_ln_modulate_fp8(*args, *rs, *common), "vcb_ln_modulate_fp8")
+    else:
+        check(lib.vcb_ln_modulate_grouped(*args, *common), "vcb_ln_modulate_grouped")
+
+
+def ln_modulate_grouped(x: torch.Tensor, out: torch.Tensor, problems: list, hidden: int, batch_rows: int, mod_stride: int, *,
+                        row_scale: torch.Tensor | None = None, stats: torch.Tensor | None = None) -> None:
+    """Two row ranges of the joint buffers in one launch.  ``problems``: two (or one) tuples (row_offset, rows, rows_per_batch, shift,
+    scale); x / out are the [*, hidden] joint buffers.  out float8_e4m3fn with ``row_scale``: the e4m3 form; ``stats``: row
+    statistics supplied by the producing GEMM (see ``_ln_launch``)."""
+    _ln_launch(x, out, problems, hidden, batch_rows, mod_stride, row_scale, stats)
 
 
 def ln_modulate_stats(x: torch.Tensor, shift: torch.Tensor, scale: torch.Tensor, out: torch.Tensor, stats: torch.Tensor,
                       rows_per_batch: int, mod_stride: int | None = None, batch_rows: int | None = None) -> torch.Tensor:
     """``ln_modulate`` with the row statistics supplied by the producing GEMM: stats [rows, n_slots, 2] fp32 (sum, sum of squares)."""
-    _req(x, BF16, "x"); _req(out, BF16, "out"); _req(stats, torch.float32, "stats"); _req(shift, BF16, "shift"); _req(scale, BF16, "scale")
-    rows, H = x.shape
-    a = _lib.LnArgs()
-    a.x, a.y, a.shift, a.scale, a.rows, a.rows_per_batch = x.data_ptr(), out.data_ptr(), shift.data_ptr(), scale.data_ptr(), rows, rows_per_batch
     ms = mod_stride if mod_stride is not None else (shift.stride(0) if shift.dim() > 1 else 0)
-    check(_lib.lib().vcb_ln_modulate_stats(C.byref(a), None, stats.data_ptr(), None, stats.shape[1], x.stride(0), out.stride(0), ms, H,
-                                           batch_rows or rows_per_batch, _stream()), "vcb_ln_modulate_stats")
+    _ln_launch(x, out, [(0, x.shape[0], rows_per_batch, shift, scale)], x.shape[1], batch_rows or rows_per_batch, ms, stats=stats)
     return out
 
 
@@ -205,20 +227,8 @@ def ln_modulate_fp8(x: torch.Tensor, shift: torch.Tensor, scale: torch.Tensor, o
                     stats: torch.Tensor | None = None) -> torch.Tensor:
     """e4m3 form of ``ln_modulate``: out8 [rows, H] float8_e4m3fn, row_scale [rows] fp32 (max|y| / 448 per row).
     ``stats`` [rows, n_slots, 2] fp32: row statistics supplied by the producing GEMM (vcb_ln_modulate_fp8_stats)."""
-    _req(x, BF16, "x"); _req(out8, torch.float8_e4m3fn, "out8"); _req(row_scale, torch.float32, "row_scale")
-    _req(shift, BF16, "shift"); _req(scale, BF16, "scale")
-    rows, H = x.shape
-    a = _lib.LnArgs()
-    a.x, a.y, a.shift, a.scale, a.rows, a.rows_per_batch = x.data_ptr(), out8.data_ptr(), shift.data_ptr(), scale.data_ptr(), rows, rows_per_batch
     ms = mod_stride if mod_stride is not None else (shift.stride(0) if shift.dim() > 1 else 0)
-    if stats is not None:
-        _req(stats, torch.float32, "stats")
-        check(_lib.lib().vcb_ln_modulate_fp8_stats(C.byref(a), None, row_scale.data_ptr(), None, stats.data_ptr(), None, stats.shape[1],
-                                                   x.stride(0), out8.stride(0), ms, H, batch_rows or rows_per_batch, _stream()),
-              "vcb_ln_modulate_fp8_stats")
-        return out8
-    check(_lib.lib().vcb_ln_modulate_fp8(C.byref(a), None, row_scale.data_ptr(), None, x.stride(0), out8.stride(0), ms, H,
-                                         batch_rows or rows_per_batch, _stream()), "vcb_ln_modulate_fp8")
+    _ln_launch(x, out8, [(0, x.shape[0], rows_per_batch, shift, scale)], x.shape[1], batch_rows or rows_per_batch, ms, row_scale, stats)
     return out8
 
 
