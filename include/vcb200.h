@@ -248,6 +248,25 @@ int vcb_rope_table(const float* ids, void* out, int32_t rows, int32_t d0, int32_
  * model_in may be NULL, else x_new is also written into its first C columns. */
 int vcb_euler_update(const void* x, const void* v, float dt_bf16, void* x_new, void* model_in, int64_t ld_in,
                      int64_t rows, int32_t C, void* stream);
+/* One stage update of torchdiffeq's fixed-grid solvers (torchdiffeq/_impl/fixed_grid.py, rk_common.py; unpinned) as
+ * transport/integrators.py:119 calls them, on one interval [t0, t1] of a bf16 state.  dt = the fp32 value of t1 - t0;
+ * v = host array of the n_v = stage + 1 model outputs v_1..v_{stage+1} of this interval, each [rows, C] bf16, where the
+ * solver's k_i = -v_i (transport.py:384).  y_out [rows, C] receives the result; model_in (may be NULL, leading dimension
+ * ld_in >= C) also receives it in columns [0, C), the rest of each row (`cond`) is left as it is.  The result equals, bit for
+ * bit, the eager torch expression with y0, k_i bf16 tensors, dt a 0-dim fp32 tensor and _one_third = 1/3 a Python float:
+ *   VCB_ODE_EULER     stage 0:  y0 + dt * k1
+ *   VCB_ODE_MIDPOINT  stage 0:  y0 + k1 * half_dt            (half_dt = 0.5 * dt; the state k2 is evaluated at)
+ *                     stage 1:  y0 + dt * k2                 (the next grid point)
+ *   VCB_ODE_RK4       stage 0:  y0 + dt * k1 * _one_third    (the 3/8 rule, rk4_alt_step_func: the state of k2)
+ *                     stage 1:  y0 + dt * (k2 - k1 * _one_third)                   (the state of k3)
+ *                     stage 2:  y0 + dt * (k1 - k2 + k3)                           (the state of k4)
+ *                     stage 3:  y0 + (k1 + 3 * (k2 + k3) + k4) * dt * 0.125       (the next grid point)
+ * 16-byte accesses when C and ld_in are multiples of 8 and every pointer is 16-byte aligned; any layout works. */
+#define VCB_ODE_EULER 0
+#define VCB_ODE_MIDPOINT 1
+#define VCB_ODE_RK4 2
+int vcb_ode_stage(int32_t method, int32_t stage, const void* y0, const void* const* v, int32_t n_v, float dt,
+                  void* y_out, void* model_in, int64_t ld_in, int64_t rows, int32_t C, void* stream);
 int vcb_copy_cols(const void* src, int64_t lds, void* dst, int64_t ldd, int32_t col0, int64_t rows, int32_t C,
                   void* stream);
 

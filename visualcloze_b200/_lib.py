@@ -73,6 +73,8 @@ _SIGNATURES = {
                                  C.c_void_p]),
     "vcb_euler_update": (C.c_int, [C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64,
                                    C.c_int32, C.c_void_p]),
+    "vcb_ode_stage": (C.c_int, [C.c_int32, C.c_int32, C.c_void_p, C.POINTER(C.c_void_p), C.c_int32, C.c_float, C.c_void_p,
+                                C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_void_p]),
     "vcb_copy_cols": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_int32,
                                 C.c_void_p]),
     "vcb_debug_umma_probe": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,

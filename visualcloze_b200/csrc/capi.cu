@@ -727,15 +727,66 @@ extern "C" int vcb_rope_table(const float* ids, void* out, int32_t rows, int32_t
     return check_launch("rope_table");
 }
 
+// One launcher for every ODE stage form (elementwise.cuh, ode_stage_kernel): 16-byte accesses when the layout allows them.
+static int ode_launch(const char* name, int form, const void* y0, const void* const* v, int n_v, float h, void* y_out,
+                      void* model_in, int64_t ld_in, int64_t rows, int32_t C, void* stream) {
+    if (!y0 || !y_out || rows <= 0 || C <= 0) return set_error("%s: bad arguments", name);
+    if (model_in && ld_in < C) return set_error("%s: ld_in (%lld) < C (%d)", name, (long long)ld_in, C);
+    OdeVs vs{};
+    uintptr_t addr_bits = (uintptr_t)y0 | (uintptr_t)y_out | (uintptr_t)model_in;
+    for (int i = 0; i < n_v; ++i) {
+        if (!v[i]) return set_error("%s: v[%d] is NULL", name, i);
+        vs.v[i] = (const __nv_bfloat16*)v[i];
+        addr_bits |= (uintptr_t)v[i];
+    }
+    if (int rc = ensure_device()) return rc;
+    const bool vec = C % 8 == 0 && (!model_in || ld_in % 8 == 0) && addr_bits % 16 == 0;
+    const long long threads = rows * C / (vec ? 8 : 1);
+    const unsigned grid = (unsigned)((threads + 255) / 256);
+    const auto* y0b = (const __nv_bfloat16*)y0;
+    auto* yo = (__nv_bfloat16*)y_out;
+    auto* mi = (__nv_bfloat16*)model_in;
+    cudaStream_t st = (cudaStream_t)stream;
+    ProfScope prof(PROF_OTHER, stream);
+#define VCB_ODE_CASE(F)                                                                                   \
+    case F:                                                                                               \
+        if (vec) ode_stage_kernel<F, 8><<<grid, 256, 0, st>>>(y0b, vs, h, yo, mi, ld_in, rows, C);         \
+        else ode_stage_kernel<F, 1><<<grid, 256, 0, st>>>(y0b, vs, h, yo, mi, ld_in, rows, C);             \
+        break;
+    switch (form) {
+        VCB_ODE_CASE(kOdeAxpy)
+        VCB_ODE_CASE(kOdeRk4K2)
+        VCB_ODE_CASE(kOdeRk4K3)
+        VCB_ODE_CASE(kOdeRk4K4)
+        VCB_ODE_CASE(kOdeRk4Final)
+        default: return set_error("%s: bad stage form %d", name, form);
+    }
+#undef VCB_ODE_CASE
+    return check_launch(name);
+}
+
+static float bf16_round_host(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
+
 extern "C" int vcb_euler_update(const void* x, const void* v, float dt_bf16, void* x_new, void* model_in, int64_t ld_in,
                                 int64_t rows, int32_t C, void* stream) {
-    if (!x || !v || !x_new || rows <= 0 || C <= 0) return set_error("euler_update: bad arguments");
-    if (int rc = ensure_device()) return rc;
-    const long long n = rows * C;
-    ProfScope prof(PROF_OTHER, stream);
-    euler_update_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
-        (const __nv_bfloat16*)x, (const __nv_bfloat16*)v, dt_bf16, (__nv_bfloat16*)x_new, (__nv_bfloat16*)model_in, ld_in, rows, C);
-    return check_launch("euler_update");
+    if (!v) return set_error("euler_update: bad arguments");
+    return ode_launch("euler_update", kOdeAxpy, x, &v, 1, dt_bf16, x_new, model_in, ld_in, rows, C, stream);
+}
+
+extern "C" int vcb_ode_stage(int32_t method, int32_t stage, const void* y0, const void* const* v, int32_t n_v, float dt,
+                             void* y_out, void* model_in, int64_t ld_in, int64_t rows, int32_t C, void* stream) {
+    static const int kForms[3][4] = {{kOdeAxpy, -1, -1, -1},
+                                     {kOdeAxpy, kOdeAxpy, -1, -1},
+                                     {kOdeRk4K2, kOdeRk4K3, kOdeRk4K4, kOdeRk4Final}};
+    if (method < VCB_ODE_EULER || method > VCB_ODE_RK4) return set_error("ode_stage: unknown method %d", method);
+    if (stage < 0 || stage > 3 || kForms[method][stage] < 0) return set_error("ode_stage: method %d has no stage %d", method, stage);
+    if (!v || n_v != stage + 1) return set_error("ode_stage: stage %d takes the %d model outputs v_1..v_%d, got n_v = %d", stage,
+                                                 stage + 1, stage + 1, n_v);
+    // midpoint: the state y0 + k1 * half_dt scales by the fp32 tensor 0.5 * dt, the final update y0 + dt * k2 reads only k2
+    const float h = bf16_round_host(method == VCB_ODE_MIDPOINT && stage == 0 ? 0.5f * dt : dt);
+    const void* const* vv = method == VCB_ODE_MIDPOINT && stage == 1 ? v + 1 : v;
+    const int nv = method == VCB_ODE_MIDPOINT && stage == 1 ? 1 : n_v;
+    return ode_launch("ode_stage", kForms[method][stage], y0, vv, nv, h, y_out, model_in, ld_in, rows, C, stream);
 }
 
 extern "C" int vcb_copy_cols(const void* src, int64_t lds, void* dst, int64_t ldd, int32_t col0, int64_t rows, int32_t C,

@@ -1,5 +1,7 @@
 // elementwise.cuh -- HBM-bound helpers of the FLUX-DiT step (coalesced 16-byte accesses, fp32 math).
 #pragma once
+#include <type_traits>
+
 #include "vcb_common.cuh"
 
 namespace vcb {
@@ -320,22 +322,67 @@ __global__ void rope_table_kernel(const float* __restrict__ ids, float2* __restr
     out[(long long)(idx % half) * rows + r] = make_float2((float)cos(ang), (float)sin(ang));
 }
 
-// Euler update (torchdiffeq fixed-grid euler via transport/integrators.py:119; SURVEY.md 8a-12):
-//   x_new = bf16(x + bf16(dt_bf16 * (-v)))   (the sampler negates the model output, transport.py:384)
-// Writes x_new to the trajectory slot and to columns [0, C) of the next model input (whose columns [C, ld_in) hold
-// the constant `cond`, transport.py:194-196).
-__global__ void euler_update_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ v,
-                                    float dt_bf16, __nv_bfloat16* __restrict__ x_new, __nv_bfloat16* __restrict__ model_in,
-                                    long long ld_in, long long rows, int C) {
-    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+// ODE stage updates of torchdiffeq's fixed-grid solvers as transport/integrators.py:119 calls them (DESIGN.md 2e).  Every
+// binary operation of the torch expression is one eager bf16 op: fp32 math on bf16 operands, one rounding r() per op.  The
+// sampler negates the model output (transport.py:384), k_i = -v_i, which is exact.  `h` is the 0-dim fp32 time-step tensor as
+// a bf16 tensor op sees it, bf16(dt) (SURVEY.md 8a-12) -- bf16(0.5 * dt) for the midpoint state; the Python-float constants
+// 1/3, 3 and 0.125 enter the fp32 op math unrounded.
+//   kOdeAxpy      r(y0 + r(h * k1))                                 euler; midpoint state (h = bf16(dt/2)) and final (k1 := k2)
+//   kOdeRk4K2     r(y0 + r(r(h * k1) * 1/3))                        rk4: y0 + dt * k1 * _one_third
+//   kOdeRk4K3     r(y0 + r(h * r(k2 - r(k1 * 1/3))))                rk4: y0 + dt * (k2 - k1 * _one_third)
+//   kOdeRk4K4     r(y0 + r(h * r(r(k1 - k2) + k3)))                 rk4: y0 + dt * (k1 - k2 + k3)
+//   kOdeRk4Final  r(y0 + r(r(h * r(r(k1 + r(3 r(k2 + k3))) + k4)) * 0.125))   rk4: y0 + (k1 + 3 * (k2 + k3) + k4) * dt * 0.125
+// The result goes to y_out (a trajectory slot or a stage buffer) and, when model_in is set, to columns [0, C) of the next model
+// input, whose columns [C, ld_in) hold the constant `cond` (transport.py:194-196).  kVec = 8: 16-byte accesses (C and ld_in
+// multiples of 8, 16-byte aligned pointers); kVec = 1 takes any layout.
+enum OdeForm : int { kOdeAxpy = 0, kOdeRk4K2, kOdeRk4K3, kOdeRk4K4, kOdeRk4Final };
+constexpr int kOdeMaxV = 4;
+
+struct OdeVs { const __nv_bfloat16* v[kOdeMaxV]; };
+
+template <int kForm>
+VCB_DEVICE float ode_stage_value(float y0, const float* k, float h) {
+    constexpr float kThird = 1.0f / 3.0f;
+    float d;
+    if constexpr (kForm == kOdeAxpy) {
+        d = bf16_round(h * k[0]);
+    } else if constexpr (kForm == kOdeRk4K2) {
+        d = bf16_round(bf16_round(h * k[0]) * kThird);
+    } else if constexpr (kForm == kOdeRk4K3) {
+        d = bf16_round(h * bf16_round(k[1] - bf16_round(k[0] * kThird)));
+    } else if constexpr (kForm == kOdeRk4K4) {
+        d = bf16_round(h * bf16_round(bf16_round(k[0] - k[1]) + k[2]));
+    } else {
+        const float s = bf16_round(3.0f * bf16_round(k[1] + k[2]));
+        const float q = bf16_round(bf16_round(k[0] + s) + k[3]);
+        d = bf16_round(bf16_round(q * h) * 0.125f);
+    }
+    return y0 + d;                                   // rounded by the caller's store
+}
+
+template <int kForm, int kVec>
+__global__ void __launch_bounds__(256) ode_stage_kernel(const __nv_bfloat16* __restrict__ y0, OdeVs vs, float h,
+                                                        __nv_bfloat16* __restrict__ y_out, __nv_bfloat16* __restrict__ model_in,
+                                                        long long ld_in, long long rows, int C) {
+    constexpr int kNv = kForm == kOdeAxpy ? 1 : kForm == kOdeRk4K2 ? 1 : kForm == kOdeRk4K3 ? 2 : kForm == kOdeRk4K4 ? 3 : 4;
+    using Pack = std::conditional_t<kVec == 8, uint4, __nv_bfloat16>;
+    const long long idx = ((long long)blockIdx.x * blockDim.x + threadIdx.x) * kVec;
     if (idx >= rows * C) return;
     const long long r = idx / C;
-    const int c = idx % C;
-    const float f = -__bfloat162float(v[idx]);
-    const float upd = bf16_round(dt_bf16 * f);
-    const __nv_bfloat16 o = __float2bfloat16_rn(__bfloat162float(x[idx]) + upd);
-    x_new[idx] = o;
-    if (model_in) model_in[r * ld_in + c] = o;
+    const int c = (int)(idx % C);
+    __nv_bfloat16 yv[kVec], vv[kNv][kVec], o[kVec];
+    *reinterpret_cast<Pack*>(yv) = *reinterpret_cast<const Pack*>(y0 + idx);
+#pragma unroll
+    for (int i = 0; i < kNv; ++i) *reinterpret_cast<Pack*>(vv[i]) = *reinterpret_cast<const Pack*>(vs.v[i] + idx);
+#pragma unroll
+    for (int j = 0; j < kVec; ++j) {
+        float k[kNv];
+#pragma unroll
+        for (int i = 0; i < kNv; ++i) k[i] = -__bfloat162float(vv[i][j]);
+        o[j] = __float2bfloat16_rn(ode_stage_value<kForm>(__bfloat162float(yv[j]), k, h));
+    }
+    *reinterpret_cast<Pack*>(y_out + idx) = *reinterpret_cast<const Pack*>(o);
+    if (model_in) *reinterpret_cast<Pack*>(model_in + r * ld_in + c) = *reinterpret_cast<const Pack*>(o);
 }
 
 // copy a [rows, C] bf16 matrix into columns [col0, col0 + C) of a wider matrix

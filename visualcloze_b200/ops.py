@@ -334,6 +334,33 @@ def euler_update(x, v, dt_bf16: float, x_new, model_in=None) -> torch.Tensor:
     return x_new
 
 
+ODE_METHODS = {"euler": 0, "midpoint": 1, "rk4": 2}          # VCB_ODE_* (include/vcb200.h)
+ODE_STAGES = {"euler": 1, "midpoint": 2, "rk4": 4}           # model evaluations per interval
+
+
+def ode_stage(method: str, stage: int, y0, vs, dt: float, y_out, model_in=None) -> torch.Tensor:
+    """One stage update of a fixed-grid solver (``vcb_ode_stage``): ``vs`` are the model outputs v_1..v_{stage+1} of the interval,
+    ``dt`` the fp32 ``t1 - t0``; writes y_out and, if given, columns [0, C) of model_in.  See include/vcb200.h for the expressions."""
+    if method not in ODE_METHODS:
+        raise ValueError(f"ode_stage: method must be one of {sorted(ODE_METHODS)}, got {method!r}")
+    _req(y0, BF16, "y0"); _req(y_out, BF16, "y_out")
+    rows, Cc = y0.shape
+    vs = [v if v.is_contiguous() else v.contiguous() for v in vs]      # e.g. a foreign model returning a column slice
+    for name, t in [("y0", y0), ("y_out", y_out)] + [(f"v[{i}]", v) for i, v in enumerate(vs)]:
+        _req(t, BF16, name)
+        if tuple(t.shape) != (rows, Cc) or t.stride(0) != Cc:
+            raise ValueError(f"ode_stage: {name} must be a dense [{rows}, {Cc}] matrix, got shape {tuple(t.shape)} strides {t.stride()}")
+    if model_in is not None:
+        _req(model_in, BF16, "model_in")
+        if model_in.shape[0] != rows or model_in.shape[1] < Cc:
+            raise ValueError(f"ode_stage: model_in must be [{rows}, >= {Cc}], got {tuple(model_in.shape)}")
+    ptrs = (C.c_void_p * max(1, len(vs)))(*[v.data_ptr() for v in vs])
+    check(_lib.lib().vcb_ode_stage(ODE_METHODS[method], stage, y0.data_ptr(), ptrs, len(vs), dt, y_out.data_ptr(),
+                                   _p(model_in), 0 if model_in is None else model_in.stride(0), rows, Cc, _stream()),
+          "vcb_ode_stage")
+    return y_out
+
+
 def copy_cols(src, dst, col0: int) -> torch.Tensor:
     _req(src, BF16, "src"); _req(dst, BF16, "dst")
     rows, Cc = src.shape

@@ -2,16 +2,18 @@
 
   create_transport  transport/__init__.py:4-62       Sampler.sample_ode  transport/transport.py:361-410
   ode grid          transport/integrators.py:79-120  time_shift          transport/utils.py:33-43
-  velocity_ode      transport/transport.py:193-198   Euler               torchdiffeq.odeint(method="euler")
+  velocity_ode      transport/transport.py:193-198   fixed-grid solvers  torchdiffeq.odeint(method="euler" | "midpoint" | "rk4")
 
 ``Sampler(transport).sample_ode(...)`` returns ``fn(x, model, model_kwargs)`` which returns the whole trajectory
 ``[num_steps, B, L, C]`` (callers index ``[-1]``).  ``num_steps`` time points mean ``num_steps - 1`` model
 evaluations.  When ``model`` is the bound ``forward`` of a ``visualcloze_b200.model.Flux`` the step-invariant work
-of all evaluations is hoisted (engine.prepare) and each step is one ``vcb_flux_forward`` + one ``vcb_euler_update``;
-any other callable is driven step by step through the same update kernel.
+of all evaluations, stage evaluations included, is hoisted (one engine.prepare) and each evaluation is one
+``vcb_flux_forward`` followed by one ``vcb_ode_stage``; any other callable is driven evaluation by evaluation through the same
+stage kernel.
 
-Only what the inference pipeline uses is implemented: Linear path, velocity prediction, fixed-grid Euler.
-Training losses, SDE samplers, likelihood ODE, VP/GVP paths and adaptive solvers are out of scope (SURVEY.md 2 #6).
+Only what the inference pipeline uses is implemented: Linear path, velocity prediction and torchdiffeq's fixed-grid solvers
+"euler", "midpoint" and "rk4" (DESIGN.md 2e).  Training losses, SDE samplers, likelihood ODE, VP/GVP paths and adaptive
+solvers are out of scope (SURVEY.md 2 #6).
 """
 from __future__ import annotations
 
@@ -96,16 +98,36 @@ def _is_native_forward(model) -> bool:
     return isinstance(getattr(model, "__self__", None), Flux) and getattr(model, "__name__", "") == "forward"
 
 
+_ONE_THIRD = 1 / 3                   # torchdiffeq/_impl/rk_common.py: _one_third, _two_thirds (Python floats)
+_TWO_THIRDS = 2 / 3
+SUPPORTED_METHODS = tuple(ops.ODE_STAGES)      # ("euler", "midpoint", "rk4")
+
+
+def stage_times(t: th.Tensor, method: str) -> th.Tensor:
+    """[N - 1, stages] fp32 solver times of every model evaluation on the grid ``t``, in evaluation order, formed by the fp32
+    tensor ops torchdiffeq applies per interval (t0, t1 0-dim fp32, dt = t1 - t0):
+      euler     t0
+      midpoint  t0, t0 + half_dt                        half_dt = 0.5 * dt              (fixed_grid.py Midpoint)
+      rk4       t0, t0 + dt * _one_third, t0 + dt * _two_thirds, t1                     (rk_common.py rk4_alt_step_func)"""
+    t0, t1 = t[:-1], t[1:]
+    dt = t1 - t0
+    cols = {"euler": lambda: [t0],
+            "midpoint": lambda: [t0, t0 + 0.5 * dt],
+            "rk4": lambda: [t0, t0 + dt * _ONE_THIRD, t0 + dt * _TWO_THIRDS, t1]}[method]()
+    return th.stack(cols, dim=1)
+
+
 class Sampler:
-    """Sampler class for the transport model (ODE / Euler only)."""
+    """Sampler class for the transport model (fixed-grid ODE solvers: euler, midpoint, rk4)."""
 
     def __init__(self, transport: Transport):
         self.transport = transport
 
     def sample_ode(self, *, sampling_method="dopri5", num_steps=50, atol=1e-6, rtol=1e-3, reverse=False, do_shift=True,
                    time_shifting_factor=None, strength=None):
-        if sampling_method != "euler":
-            raise NotImplementedError("only the fixed-grid 'euler' solver (the pipeline default, visualcloze.py:81) is implemented")
+        if sampling_method not in SUPPORTED_METHODS:
+            raise NotImplementedError(f"sampling_method={sampling_method!r}: only the fixed-grid solvers "
+                                      f"{', '.join(map(repr, SUPPORTED_METHODS))} are implemented (adaptive solvers are not)")
         t0, t1 = self.transport.check_interval(self.transport.train_eps, self.transport.sample_eps, sde=False, eval=True,
                                                reverse=reverse, last_step_size=0.0)
         if strength is not None:
@@ -113,32 +135,34 @@ class Sampler:
         assert t0 < t1, "ODE sampler has to be in forward time"
 
         def _sample(x, model, model_kwargs):
-            return _euler_sample(x, model, model_kwargs, t0, t1, num_steps, do_shift, time_shifting_factor)
+            return _fixed_grid_sample(x, model, model_kwargs, sampling_method, t0, t1, num_steps, do_shift, time_shifting_factor)
 
         return _sample
 
 
-def _euler_sample(x, model, model_kwargs, t0, t1, num_steps, do_shift, time_shifting_factor):
+def _fixed_grid_sample(x, model, model_kwargs, method, t0, t1, num_steps, do_shift, time_shifting_factor):
     if not (x.is_cuda and x.dtype == th.bfloat16):
         raise ops._lib.VcbError("the sampler runs on CUDA bf16 latents only (visualcloze.py:399); there is no CPU path")
     B, Li, C = x.shape
     t = solver_grid(t0, t1, num_steps, Li, do_shift, time_shifting_factor)
-    n_eval = int(num_steps) - 1
+    n_int = int(num_steps) - 1
+    stages = ops.ODE_STAGES[method]
+    n_eval = stages * n_int                       # evaluation e = k * stages + s: stage s of interval k
     kw = dict(model_kwargs)                       # the caller's dict is not mutated (transport.py:194-196 pops a copy)
     cond = kw.pop("cond", None)
     # FLUX time fed to the model: ones(B) * t -> 1 - t (integrators.py:109, transport.py:384), fp32.  torchdiffeq wraps the
     # ODE function in _PerturbFunc, which casts the evaluation time to the STATE dtype (t.to(y.abs().dtype)): with the bf16
-    # latent the model sees 1 - bf16(tau_k) (up to ~2 units of 1000 t near tau = 1).  dt keeps the fp32 grid.
-    t_vec = th.ones(n_eval, B) * t[:-1, None].to(x.dtype).float()
+    # latent the model sees 1 - bf16(tau) (up to ~2 units of 1000 t near tau = 1).  The stage times are fp32 ops on the grid.
+    t_vec = th.ones(n_eval, B) * stage_times(t, method).reshape(n_eval, 1).to(x.dtype).float()
     flux_t = th.ones_like(t_vec) * (1 - t_vec)
-    # dt is a 0-dim fp32 tensor multiplied into a bf16 tensor: it acts as a bf16 scalar (SURVEY.md 8a-12)
-    dts = [float((t[k + 1] - t[k]).to(th.bfloat16)) for k in range(n_eval)]
+    # dt is the fp32 t1 - t0; the stage kernel applies it as torch does a 0-dim fp32 tensor in a bf16 op (vcb_ode_stage)
+    dts = [float(t[k + 1] - t[k]) for k in range(n_int)]
 
     native = _is_native_forward(model)
     sp = model.__self__.engine()._sp if native else None
     if sp is not None:
-        # single-image sequence parallelism: this rank integrates its own token rows (the ODE is row-local apart from the
-        # attention inside the model); the trajectory is gathered once at the end.  The time grid above used the FULL Li.
+        # single-image sequence parallelism: this rank integrates its own token rows (every stage update is row-local; only
+        # the attention inside the model mixes rows); the trajectory is gathered once at the end.  The grid used the FULL Li.
         x = sp.shard(x).contiguous()
         cond = None if cond is None else sp.shard(cond)
     Li_full, Li = Li, x.shape[1]
@@ -149,6 +173,7 @@ def _euler_sample(x, model, model_kwargs, t0, t1, num_steps, do_shift, time_shif
     ops.copy_cols(traj[0].reshape(B * Li, C), inp.reshape(B * Li, C + Cc), 0)
     if cond is not None:
         ops.copy_cols(cond.to(x.dtype).reshape(B * Li, Cc).contiguous(), inp.reshape(B * Li, C + Cc), C)
+    y_stage = th.empty(B * Li, C, dtype=x.dtype, device=x.device) if stages > 1 else None   # stage states are not returned
 
     if native:
         flux = model.__self__
@@ -157,16 +182,19 @@ def _euler_sample(x, model, model_kwargs, t0, t1, num_steps, do_shift, time_shif
             raise ValueError("Didn't get guidance strength for guidance distilled model.")
         eng.prepare(txt=kw["txt"], y=kw["y"], img_ids=kw["img_ids"], txt_ids=kw["txt_ids"], timesteps=flux_t,
                     guidance=kw.get("guidance"), txt_mask=kw.get("txt_mask"), img_mask=kw.get("img_mask"), n_img_tokens=Li_full)
-        v = th.empty(B, Li, flux.params.out_channels, dtype=x.dtype, device=x.device)
-    for k in range(n_eval):
-        if native:
-            eng.forward(k, inp, v)
-            out = v
-        else:
-            out = model(inp, timesteps=flux_t[k].to(x.device), **kw)
-        assert out.shape == x.shape, "Output shape from ODE solver must match input shape"
-        ops.euler_update(traj[k].reshape(B * Li, C), out.reshape(B * Li, C), dts[k], traj[k + 1].reshape(B * Li, C),
-                         inp.reshape(B * Li, C + Cc))
+        v = th.empty(stages, B, Li, flux.params.out_channels, dtype=x.dtype, device=x.device)
+    for k in range(n_int):
+        vs = []
+        for s in range(stages):
+            e = k * stages + s
+            if native:
+                out = eng.forward(e, inp, v[s])
+            else:
+                out = model(inp, timesteps=flux_t[e].to(x.device), **kw)
+            assert out.shape == x.shape, "Output shape from ODE solver must match input shape"
+            vs.append(out.reshape(B * Li, C))
+            y_out = traj[k + 1].reshape(B * Li, C) if s == stages - 1 else y_stage
+            ops.ode_stage(method, s, traj[k].reshape(B * Li, C), vs, dts[k], y_out, inp.reshape(B * Li, C + Cc))
     if sp is not None:
         traj = sp.gather(traj, dim=2)
         sp.check()
