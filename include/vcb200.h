@@ -38,7 +38,8 @@ int         vcb_profile_begin(void);
 int         vcb_profile_end(double ms[4], long long launches[4]);
 /* Extended form: ncat in [4, 6] categories (4 = VAE 3x3 convolutions, 5 = VAE GroupNorm / upsample / softmax / layout; with
  * ncat == 4 they fold into "other"), and optionally one record per launch in launch order.
- * info: GEMM {M, N, K, epilogue | (block_n / 32) << 8 | cta_group << 16 | issued-by-the-VAE-engine << 24}; conv {output pixels, cout, 9 * cin, stride};
+ * info: GEMM {M, N, K, epilogue | (block_n / 32) << 8 | cta_group << 16 | issued-by-the-VAE-engine << 24 | stream-K tail taken << 25};
+ * conv {output pixels, cout, 9 * cin, stride};
  * attention {B, L, heads, fixed-reference softmax | persistent schedule << 1}. */
 typedef struct vcb_prof_record { int32_t category; float ms; int32_t info[4]; } vcb_prof_record;
 int         vcb_profile_end_ex(double* ms, long long* launches, int32_t ncat, vcb_prof_record* records, int64_t capacity,
@@ -56,7 +57,9 @@ enum vcb_epilogue {
     VCB_EPI_LINEAR1 = 4,   /* cols < 3H as QKV -> out; cols >= 3H as BIAS_GELU -> out2     layers.py:235-244 */
     VCB_EPI_BIAS_F32 = 5   /* out is FP32 [.., ldo]: acc + bias (VAE attention scores, autoencoder.py:47) */
 };
-/* VCB_EPI_GATE_RES with gate == NULL is the ungated residual out = bf16(res + bf16(acc + bias)). */
+/* VCB_EPI_GATE_RES with gate == NULL is the ungated residual out = bf16(res + bf16(acc + bias)).
+ * N % 8 != 0 (VCB_EPI_BIAS / VCB_EPI_BIAS_F32 only): the columns past N up to round_up(N, 8) (bf16 out) or round_up(N, 4) (fp32
+ * out) are written too, with the epilogue of a zero accumulator without bias: +0.  Nothing else outside the problem is written. */
 
 typedef struct vcb_gemm_args {
     int32_t M, N, K;
@@ -127,13 +130,14 @@ int vcb_gemm_bf16_grouped(const vcb_gemm_args* args0, const vcb_gemm_args* args1
  * filter tap's shift, zero-filled outside the image.  x [n,H,W,cin], w [cout, 3,3,cin] (tap-major, channels last),
  * out [n,H/stride,W/stride,cout]; res (optional, same shape as out): out = bf16(res + bf16(conv + bias)).
  * stride 1: zero padding 1 all round.  stride 2: the encoder's Downsample (autoencoder.py:85-95): pad right/bottom by 1,
- * no padding left/top; the TMA map carries elementStrides = 2.  cin % 64 == 0, cout % 8 == 0. */
+ * no padding left/top; the TMA map carries elementStrides = 2; H and W even.  cin % 64 == 0, cout % 8 == 0. */
 int vcb_conv3x3_nhwc(const void* x, const void* w, const float* bias, const void* res, void* out, int32_t n,
                      int32_t H, int32_t W, int32_t cin, int32_t cout, int32_t stride, void* stream);
 
 /* ---- joint attention (models/math.py:63-99: attention/_upad_input/flash_attn_varlen_func/pad_input) ------
  * qkv: [B, L, ld_qkv] bf16, head h of q/k/v at columns {q,k,v}_col + 128*h, RoPE + QK-norm already applied.
- * seqlens: [B] int32 valid tokens (right padding) or NULL.  out rows >= seqlen are written as zeros. */
+ * seqlens: [B] int32 valid tokens (right padding) or NULL.  out rows >= seqlen are written as +0.  The padded rows of qkv
+ * (rows >= seqlen of a sample) may hold any bytes, non-finite values included: they never reach a valid output row. */
 int vcb_attention_fwd(const void* qkv, int64_t ld_qkv, int32_t q_col, int32_t k_col, int32_t v_col,
                       const int32_t* seqlens, int32_t B, int32_t L, int32_t heads,
                       void* out, int64_t ldo, int32_t out_col_offset, void* stream);

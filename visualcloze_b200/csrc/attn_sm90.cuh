@@ -300,6 +300,20 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const AttnPa
                 }
                 // ---- O (+)= P V_j: V is MN-major (head dim contiguous): two [128 keys x 64] blocks, 16 keys = 2048 bytes ----
                 mbar_wait(&kv_full[v_slot], (uint32_t)((seq + 1) / kAttnSlots) & 1u);
+                // Padded keys of a right-padded sample's last tile: their P entries are exactly 0, but the tensor core's 0 * NaN and
+                // 0 * Inf are NaN, and the padded V rows hold whatever the caller left there (they lie inside L, so the TMA unit loads
+                // them; rows >= L arrive zero-filled).  Zero them first: whole 128-byte rows of both 64-column blocks, independent of
+                // the swizzle.  Both warpgroups read the slot, so both take part and meet at a barrier after the proxy fence.
+                if (kv_left < kAttnTile && seqlen < p.L) {
+                    const int n_pad = min(kAttnTile, p.L - j * kAttnTile) - kv_left;           // uint4 per row: 8
+                    uint4* vs = reinterpret_cast<uint4*>(smem_kv + v_slot * kSlotBytes);
+                    for (int i = ctid; i < 2 * n_pad * 8; i += kAttnConsumers) {
+                        const int half = i / (n_pad * 8), r = i - half * (n_pad * 8);
+                        vs[half * (kSlotBytes / 32) + (kv_left + (r >> 3)) * 8 + (r & 7)] = make_uint4(0, 0, 0, 0);
+                    }
+                    fence_proxy_async_smem();                       // generic-proxy stores -> visible to the wgmma (async proxy)
+                    named_bar_sync(1, kAttnConsumers);
+                }
                 const uint64_t vd = make_smem_desc(smem_u32(smem_kv + v_slot * kSlotBytes), kSlotBytes / 2, 1024);
                 wgmma_fence();
 #pragma unroll
@@ -375,9 +389,11 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const AttnPa
                         frag_row8(o, c, h, q, v);
                         const int row = q0 + frag_row + 8 * h;
                         if (row < p.L) {
-                            const float inv_l = row < seqlen ? 1.0f / l_run[h] : 0.f;      // padded query rows: zeros (pad_input)
+                            // padded query rows: +0 (pad_input) as a select -- their o may be NaN when Q holds NaN there
+                            const bool valid = row < seqlen;
+                            const float inv_l = 1.0f / l_run[h];
 #pragma unroll
-                            for (int i = 0; i < 8; ++i) v[i] *= inv_l;
+                            for (int i = 0; i < 8; ++i) v[i] = valid ? v[i] * inv_l : 0.f;
                             store_bf16x8(attn_out_row(p, b, row) + p.out_col_offset + head * 128 + c * 32 + 8 * (int)q, v);
                         }
                     }

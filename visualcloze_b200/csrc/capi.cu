@@ -64,6 +64,12 @@ inline bool streamk_wanted(long tiles, int slots, float tile_us) {
     return mode == 1 || idle / waves >= 0.2f;
 }
 
+// whether the calling thread's most recent GEMM launch took the stream-K tail (marked in its profile record, vcb200.h)
+inline bool& gemm_streamk_taken() {
+    static thread_local bool taken = false;
+    return taken;
+}
+
 template <int BN, int CG, int EPI, bool SP = false, bool FP8 = false>
 int launch_gemm_inst(const Problem& g0, const Problem& g1, float rate, cudaStream_t st) {
     const CUtensorMap& ta = g0.ta; const CUtensorMap& tb = g0.tb; const GemmParams& p = g0.p;
@@ -83,6 +89,7 @@ int launch_gemm_inst(const Problem& g0, const Problem& g1, float rate, cudaStrea
     // stream-K tail: the tiles of the partial last wave are cut along K into one equal range per CTA (pair)
     StreamKParams skp{nullptr, nullptr, 0, 0};
     const bool sk = streamk_wanted(tiles, clusters, tile_time_us(BN, p.K + p.lora_rank, rate) * (FP8 ? 0.5f : 1.0f));
+    gemm_streamk_taken() = sk;
     if (tiles < clusters && !sk) clusters = tiles;
     if (sk) {
         SkScratch* sc = sk_scratch(st);
@@ -280,7 +287,12 @@ int gemm_dispatch(const vcb_gemm_args* a, const vcb_gemm_args* a1, void* stream)
     const bool stats = a->row_stats || (a1 && a1->row_stats);      // 64-column statistics slots: tiles of 128 or 256 columns
     pick_tile(batch, a->rows_per_batch + (a1 ? a1->M / batch : 0), a->N, a->K + a->lora_rank, head || fp8 || stats, a->cta_group ? a->cta_group : forced_cta_group(),
               a->block_n, &cg, &bn, &rate);
-    ProfScope prof(PROF_GEMM, stream, a->M + (a1 ? a1->M : 0), a->N, a->K, a->epilogue | ((bn >> 5) << 8) | (cg << 16));
+    const int info3 = a->epilogue | ((bn >> 5) << 8) | (cg << 16);
+    ProfScope prof(PROF_GEMM, stream, a->M + (a1 ? a1->M : 0), a->N, a->K, info3);
+    auto mark_streamk = [&](int rc) {
+        if (rc == 0 && gemm_streamk_taken()) prof.set_info(3, info3 | (prof_context() << 24) | (1 << 25));
+        return rc;
+    };
     Problem g0, g1;
     if (int rc = build_problem(a, bn, cg, &g0)) return rc;
     if (a1) {
@@ -300,7 +312,7 @@ int gemm_dispatch(const vcb_gemm_args* a, const vcb_gemm_args* a1, void* stream)
     cudaStream_t st = (cudaStream_t)stream;
     if (fp8) {
 #define VCB_GEMM_CASE8(BN, CG) \
-    if (bn == BN && cg == CG) return launch_gemm_epi_fp8<BN, CG>(a->epilogue, g0, g1, rate, st);
+    if (bn == BN && cg == CG) return mark_streamk(launch_gemm_epi_fp8<BN, CG>(a->epilogue, g0, g1, rate, st));
         VCB_GEMM_CASE8(128, 1)
         VCB_GEMM_CASE8(256, 1)
         VCB_GEMM_CASE8(128, 2)
@@ -309,7 +321,7 @@ int gemm_dispatch(const vcb_gemm_args* a, const vcb_gemm_args* a1, void* stream)
         return set_error("gemm (fp8): unsupported (block_n=%d, cta_group=%d)", bn, cg);
     }
 #define VCB_GEMM_CASE(BN, CG) \
-    if (bn == BN && cg == CG) return launch_gemm_epi<BN, CG>(a->epilogue, g0, g1, rate, st);
+    if (bn == BN && cg == CG) return mark_streamk(launch_gemm_epi<BN, CG>(a->epilogue, g0, g1, rate, st));
     VCB_GEMM_CASE(64, 1)
     VCB_GEMM_CASE(128, 1)
     VCB_GEMM_CASE(192, 1)

@@ -8,7 +8,7 @@ import torch
 from . import _lib
 from ._lib import GemmArgs, check
 
-EPI_BIAS, EPI_BIAS_GELU, EPI_GATE_RES, EPI_QKV, EPI_LINEAR1 = range(5)
+EPI_BIAS, EPI_BIAS_GELU, EPI_GATE_RES, EPI_QKV, EPI_LINEAR1, EPI_BIAS_F32 = range(6)
 BF16 = torch.bfloat16
 
 
@@ -63,7 +63,8 @@ def gemm_args(a: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None, out: 
         _req(a, torch.float8_e4m3fn, "a"); _req(w, torch.float8_e4m3fn, "w")
     else:
         _req(a, BF16, "a"); _req(w, BF16, "w")
-    _req(out, BF16, "out")
+    # EPI_BIAS_F32: fp32 out = acc + bias, bf16 operands only (the library refuses e4m3 operands for it)
+    _req(out, torch.float32 if epilogue == EPI_BIAS_F32 and not fp8 else BF16, "out")
     M, K = a.shape
     if m is not None:
         M = m
