@@ -274,6 +274,23 @@ int vcb_ode_stage(int32_t method, int32_t stage, const void* y0, const void* con
 int vcb_copy_cols(const void* src, int64_t lds, void* dst, int64_t ldd, int32_t col0, int64_t rows, int32_t C,
                   void* stream);
 
+/* ---- grid-cell preparation (visualcloze.py:300-360, 133-137, 200): bit-exact to Pillow's Image.resize of an RGB image
+ * (LANCZOS / BICUBIC, reducing_gap=None) and to image_transform.  Images are interleaved uint8 [h][w][3] with a row stride in
+ * BYTES. ----------------------------------------------------------------------------------------------------------------- */
+/* One pass of Pillow's 8-bit resampler along axis 0 (x: out [in_h][out_n][3]) or 1 (y: out [out_n][in_w][3]).  bounds
+ * [out_n][2] int32 (xmin, n) and coeffs [out_n][ksize] int32 are device arrays, Pillow's precompute_coeffs +
+ * normalize_coeffs_8bpc (22 fractional bits); out = clamp((2^21 + sum_k coeffs[i][k] * in[xmin + k]) >> 22, 0, 255) in int32.
+ * The window of a sample is clipped to the input and to ksize taps (a correct table never needs the clip).  A resize is the
+ * x pass, then the y pass on its uint8 output; Pillow skips the pass of an axis whose size does not change. */
+int vcb_resample_u8(const void* in, int64_t in_ld, int32_t in_w, int32_t in_h, int32_t axis, const int32_t* bounds,
+                    const int32_t* coeffs, int32_t ksize, int32_t out_n, void* out, int64_t out_ld, void* stream);
+/* The crop box (crop_x, crop_y, crop_w, crop_h) of a uint8 image -> fp32 planes out[c * out_ld_plane + y * out_ld_row + col0 + x]
+ * = (u / 255 - 0.5) / 0.5 with fp32 division and subtraction (torchvision ToTensor + Normalize(0.5, 0.5)).  Box pixels outside
+ * the image are 0, as Image.crop pads them, and become -1; in_w = 0 or in_h = 0 (in may be NULL) is a blank cell. */
+int vcb_u8_to_model_input(const void* in, int64_t in_ld, int32_t in_w, int32_t in_h, int32_t crop_x, int32_t crop_y,
+                          int32_t crop_w, int32_t crop_h, float* out, int64_t out_ld_row, int64_t out_ld_plane, int32_t col0,
+                          void* stream);
+
 
 /* ---- FLUX-DiT engine: the whole Flux.forward (models/model.py:85-124) and the Euler loop around it -----------
  * Weights are the reference's tensors in one of two forms, chosen per Linear (lora.py:92-98): LoRA merged (rank 0:

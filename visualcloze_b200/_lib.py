@@ -77,6 +77,10 @@ _SIGNATURES = {
                                 C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_void_p]),
     "vcb_copy_cols": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_int32,
                                 C.c_void_p]),
+    "vcb_resample_u8": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32,
+                                  C.c_int32, C.c_void_p, C.c_int64, C.c_void_p]),
+    "vcb_u8_to_model_input": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                        C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_void_p]),
     "vcb_debug_umma_probe": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
                                        C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p]),
 }

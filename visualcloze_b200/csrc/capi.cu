@@ -13,6 +13,7 @@
 #include "gemm_sm90.cuh"
 #include "host_util.cuh"
 #include "probe.cuh"
+#include "resample.cuh"
 #include "sp_sm90.cuh"
 
 using namespace vcb;
@@ -810,6 +811,54 @@ extern "C" int vcb_copy_cols(const void* src, int64_t lds, void* dst, int64_t ld
     copy_cols_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
         (const __nv_bfloat16*)src, lds, (__nv_bfloat16*)dst, ldd, col0, rows, C);
     return check_launch("copy_cols");
+}
+
+// ------------------------------------------------------------------------------------------------
+// grid-cell preparation (resample.cuh)
+// ------------------------------------------------------------------------------------------------
+extern "C" int vcb_resample_u8(const void* in, int64_t in_ld, int32_t in_w, int32_t in_h, int32_t axis, const int32_t* bounds,
+                               const int32_t* coeffs, int32_t ksize, int32_t out_n, void* out, int64_t out_ld, void* stream) {
+    if (!in || !out || !bounds || !coeffs) return set_error("resample_u8: null pointer");
+    if (axis != 0 && axis != 1) return set_error("resample_u8: axis must be 0 (x) or 1 (y), got %d", axis);
+    if (in_w < 1 || in_h < 1 || out_n < 1) return set_error("resample_u8: bad sizes (in %d x %d, out_n %d)", in_w, in_h, out_n);
+    if (ksize < 1) return set_error("resample_u8: ksize must be >= 1, got %d", ksize);
+    const int out_w = axis == 0 ? out_n : in_w;
+    if (in_ld < 3LL * in_w || out_ld < 3LL * out_w)
+        return set_error("resample_u8: row strides (in %lld, out %lld bytes) must hold 3 * width bytes", (long long)in_ld,
+                         (long long)out_ld);
+    if (int rc = ensure_device()) return rc;
+    const long long n = (long long)out_w * (axis == 0 ? in_h : out_n);
+    ProfScope prof(PROF_OTHER, stream);
+    const unsigned grid = (unsigned)((n + 255) / 256);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (axis == 0)
+        resample_u8_kernel<0><<<grid, 256, 0, st>>>((const uint8_t*)in, in_ld, in_w, in_h, bounds, coeffs, ksize, out_n,
+                                                    (uint8_t*)out, out_ld);
+    else
+        resample_u8_kernel<1><<<grid, 256, 0, st>>>((const uint8_t*)in, in_ld, in_w, in_h, bounds, coeffs, ksize, out_n,
+                                                    (uint8_t*)out, out_ld);
+    return check_launch("resample_u8");
+}
+
+extern "C" int vcb_u8_to_model_input(const void* in, int64_t in_ld, int32_t in_w, int32_t in_h, int32_t crop_x, int32_t crop_y,
+                                     int32_t crop_w, int32_t crop_h, float* out, int64_t out_ld_row, int64_t out_ld_plane,
+                                     int32_t col0, void* stream) {
+    if (!out) return set_error("u8_to_model_input: null output");
+    if (in_w < 0 || in_h < 0 || crop_w < 1 || crop_h < 1 || col0 < 0)
+        return set_error("u8_to_model_input: bad sizes (in %d x %d, crop %d x %d, col0 %d)", in_w, in_h, crop_w, crop_h, col0);
+    const bool empty = in_w == 0 || in_h == 0;
+    if (!empty && !in) return set_error("u8_to_model_input: null input");
+    if (!empty && in_ld < 3LL * in_w) return set_error("u8_to_model_input: in_ld (%lld) < 3 * in_w", (long long)in_ld);
+    if (out_ld_row < (int64_t)col0 + crop_w || out_ld_plane < (int64_t)crop_h * out_ld_row)
+        return set_error("u8_to_model_input: the output planes (ld_row %lld, ld_plane %lld) do not hold %d x %d at column %d",
+                         (long long)out_ld_row, (long long)out_ld_plane, crop_h, crop_w, col0);
+    if (int rc = ensure_device()) return rc;
+    const long long n = (long long)crop_w * crop_h;
+    ProfScope prof(PROF_OTHER, stream);
+    cell_to_model_input_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+        empty ? nullptr : (const uint8_t*)in, in_ld, empty ? 0 : in_w, empty ? 0 : in_h, crop_x, crop_y, crop_w, crop_h, out,
+        out_ld_row, out_ld_plane, col0);
+    return check_launch("u8_to_model_input");
 }
 
 // ------------------------------------------------------------------------------------------------

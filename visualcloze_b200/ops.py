@@ -370,6 +370,52 @@ def copy_cols(src, dst, col0: int) -> torch.Tensor:
     return dst
 
 
+def _req_image(img: torch.Tensor, name: str):
+    """uint8 [h, w, 3] CUDA tensor with dense pixels (any row stride)"""
+    _req(img, torch.uint8, name)
+    if img.dim() != 3 or img.shape[2] != 3 or img.stride(1) != 3:
+        raise _lib.VcbError(f"{name} must be a uint8 [h, w, 3] image with interleaved pixels, got shape {tuple(img.shape)} "
+                            f"strides {img.stride()}")
+
+
+def resample_u8(img: torch.Tensor, axis: int, bounds: torch.Tensor, coeffs: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
+    """One pass of Pillow's 8-bit resampler (``vcb_resample_u8``) along axis 0 (x) or 1 (y): img / out uint8 [h, w, 3] images,
+    bounds [out_n, 2] / coeffs [out_n, ksize] int32 tables (``resample.coeffs_8bpc``) built for img's length along the axis."""
+    _req_image(img, "img"); _req_image(out, "out"); _req(bounds, torch.int32, "bounds"); _req(coeffs, torch.int32, "coeffs")
+    out_n, ksize = coeffs.shape
+    if not (bounds.is_contiguous() and coeffs.is_contiguous() and tuple(bounds.shape) == (out_n, 2)):
+        raise _lib.VcbError(f"resample_u8: bounds [out_n, 2] and coeffs [out_n, ksize] must be dense, got {tuple(bounds.shape)}, "
+                            f"{tuple(coeffs.shape)}")
+    h, w = img.shape[0], img.shape[1]
+    want = (h, out_n) if axis == 0 else (out_n, w)
+    if tuple(out.shape[:2]) != want:
+        raise _lib.VcbError(f"resample_u8: out must be [{want[0]}, {want[1]}, 3], got {tuple(out.shape)}")
+    check(_lib.lib().vcb_resample_u8(img.data_ptr(), img.stride(0), w, h, axis, bounds.data_ptr(), coeffs.data_ptr(), ksize, out_n,
+                                     out.data_ptr(), out.stride(0), _stream()), "vcb_resample_u8")
+    return out
+
+
+def u8_to_model_input(img: torch.Tensor | None, box, out: torch.Tensor, col0: int) -> torch.Tensor:
+    """``vcb_u8_to_model_input``: the crop ``box`` = (left, top, right, bottom) of img (uint8 [h, w, 3], or None for a blank cell)
+    as ``image_transform`` values into out[:, :, col0:col0 + width] (out fp32 [3, H, W], dense rows); box pixels outside img
+    are -1."""
+    _req(out, torch.float32, "out")
+    if out.dim() != 3 or out.shape[0] != 3:
+        raise _lib.VcbError(f"out must be fp32 [3, H, W], got {tuple(out.shape)}")
+    left, top, right, bottom = box
+    if col0 < 0 or out.shape[2] < col0 + right - left or out.shape[1] < bottom - top:
+        raise _lib.VcbError(f"u8_to_model_input: a {right - left} x {bottom - top} box at column {col0} does not fit "
+                            f"out {tuple(out.shape)}")
+    if img is None:
+        ptr, ld, w, h = None, 0, 0, 0
+    else:
+        _req_image(img, "img")
+        ptr, ld, w, h = img.data_ptr(), img.stride(0), img.shape[1], img.shape[0]
+    check(_lib.lib().vcb_u8_to_model_input(ptr, ld, w, h, left, top, right - left, bottom - top, out.data_ptr(), out.stride(1),
+                                           out.stride(0), col0, _stream()), "vcb_u8_to_model_input")
+    return out
+
+
 def umma_probe(a, b, ksteps: int, b_mn_major: bool, a_from_regs: bool, b_lbo: int = 0, b_sbo: int = 0,
                b_kstep_bytes: int = 0) -> torch.Tensor:
     out = torch.empty(128, 128, dtype=torch.float32, device=a.device)

@@ -18,11 +18,13 @@ row-wise RoPE ids, sampler settings and output cropping.  What differs is where 
 from __future__ import annotations
 
 import random
+from typing import NamedTuple
 
 import numpy as np
 import torch
 from PIL import Image
 
+from . import ops, resample
 from .model import FluxLoraWrapper, flux_dev_fill_params
 from .sampling import prepare_modified
 from .transport import Sampler, create_transport
@@ -38,23 +40,21 @@ _CONTENT_PREFIXES = (
 )
 
 
-def resize_with_aspect_ratio(img: Image.Image, resolution: int, divisible: int = 16, aspect_ratio=None) -> Image.Image:
-    """area ~= resolution^2, aspect kept, both sides multiples of 16 (visualcloze.py:28-75, PIL branch)."""
-    w, h = img.size
+def aspect_ratio_size(size, resolution: int, divisible: int = 16, aspect_ratio=None) -> tuple:
+    """The size ``resize_with_aspect_ratio`` resizes an image of ``size`` = (w, h) to."""
+    w, h = size
     if aspect_ratio is None:
         aspect_ratio = w / h
     new_h = int((resolution * resolution / aspect_ratio) ** 0.5)
     new_w = int(new_h * aspect_ratio)
     new_w = max(new_w // divisible, 1) * divisible
     new_h = max(new_h // divisible, 1) * divisible
-    return img.resize((new_w, new_h), Image.LANCZOS)
+    return new_w, new_h
 
 
-def center_crop(image: Image.Image, target_size) -> Image.Image:
-    w, h = image.size
-    nw, nh = target_size
-    left, top = (w - nw) // 2, (h - nh) // 2
-    return image.crop((left, top, left + nw, top + nh))
+def resize_with_aspect_ratio(img: Image.Image, resolution: int, divisible: int = 16, aspect_ratio=None) -> Image.Image:
+    """area ~= resolution^2, aspect kept, both sides multiples of 16 (visualcloze.py:28-75, PIL branch)."""
+    return img.resize(aspect_ratio_size(img.size, resolution, divisible, aspect_ratio), Image.LANCZOS)
 
 
 def to_rgb_if_rgba(img: Image.Image) -> Image.Image:
@@ -85,6 +85,91 @@ def _patchify(lat: torch.Tensor) -> torch.Tensor:
     """"b c (h ph)(w pw) -> b (h w)(c ph pw)", ph = pw = 2."""
     b, c, H, W = lat.shape
     return lat.reshape(b, c, H // 2, 2, W // 2, 2).permute(0, 2, 4, 1, 3, 5).reshape(b, (H // 2) * (W // 2), c * 4)
+
+
+class CellPlan(NamedTuple):
+    """How one grid cell is made: start from the caller's image (``blank`` None) or from a black RGB image of size ``blank``
+    (a missing target), then apply ``ops`` in order: ("resize", (w, h), filter) with filter ``resample.LANCZOS`` /
+    ``resample.BICUBIC``, or ("crop", (left, top, right, bottom)) with Pillow's zero padding outside the image."""
+    blank: tuple | None
+    ops: tuple
+
+    @property
+    def size(self) -> tuple:
+        """(w, h) of the finished cell"""
+        if not self.ops:
+            return self.blank
+        op = self.ops[-1]
+        return op[1] if op[0] == "resize" else (op[1][2] - op[1][0], op[1][3] - op[1][1])
+
+
+def grid_plan(sizes, grid_h: int, grid_w: int, resolution: int):
+    """The decisions of visualcloze.py:300-360 as a pure function of the input sizes, with the reference's quirks (the
+    multi-target loop reassigns ``new_w``).  sizes[i][j]: (w, h) of cell (i, j), or None for a missing target of the last row.
+    -> (cells: CellPlan per cell, row-major; mask_position; upsampling_size)."""
+    cells, mask_position = [], []
+    target_size = upsampling_size = None
+    for i in range(grid_h):
+        reference_size = None
+        for j in range(grid_w):
+            if sizes[i][j] is not None:
+                if i == grid_h - 1 and upsampling_size is None:
+                    upsampling_size = tuple(sizes[i][j])
+                reference_size = aspect_ratio_size(sizes[i][j], resolution)
+                if i == grid_h - 1 and target_size is None:
+                    target_size = reference_size
+                break
+        for j in range(grid_w):
+            if sizes[i][j] is not None:
+                tw, th = aspect_ratio_size(sizes[i][j], resolution)
+                if tw <= th:
+                    size = (reference_size[0], int(reference_size[0] / tw * th))
+                else:
+                    size = (int(reference_size[1] / th * tw), reference_size[1])
+                left, top = (size[0] - reference_size[0]) // 2, (size[1] - reference_size[1]) // 2      # center_crop
+                cells.append(CellPlan(None, (("resize", (tw, th), resample.LANCZOS), ("resize", size, resample.BICUBIC),
+                                             ("crop", (left, top, left + reference_size[0], top + reference_size[1])))))
+                if i == grid_h - 1:
+                    mask_position.append(0)
+            else:
+                if i != grid_h - 1:
+                    raise ValueError("Please provide each image in the in-context example.")
+                cells.append(CellPlan(reference_size or (resolution, resolution), ()))
+                mask_position.append(1)
+    if len(mask_position) > 1 and sum(mask_position) > 1:
+        new_w = 384 if target_size is None else target_size[0]
+        for k, cell in enumerate(cells):
+            w, h = cell.size
+            new_h = int(h * (new_w / w))
+            new_w, new_h = int(new_w / 16) * 16, int(new_h / 16) * 16
+            cells[k] = cell._replace(ops=cell.ops + (("resize", (new_w, new_h), resample.BICUBIC),))
+    return cells, mask_position, upsampling_size
+
+
+_PIL_FILTERS = {resample.LANCZOS: Image.LANCZOS, resample.BICUBIC: Image.BICUBIC}
+
+
+def run_cell_pil(image, cell: CellPlan) -> Image.Image:
+    """One CellPlan executed with Pillow."""
+    im = image if cell.blank is None else Image.new("RGB", cell.blank, (0, 0, 0))
+    for op in cell.ops:
+        im = im.resize(op[1], _PIL_FILTERS[op[2]]) if op[0] == "resize" else im.crop(op[1])
+    return im
+
+
+def run_cell_device(image: torch.Tensor | None, cell: CellPlan, out: torch.Tensor, col0: int) -> None:
+    """One CellPlan executed on the device: image uint8 [h, w, 3] CUDA (None for a blank cell) -> ``image_transform`` of the
+    cell into out[:, :, col0:col0 + w] (out fp32 [3, h, W]).  A crop that ends the plan is done by the store."""
+    im, ops_ = image, cell.ops
+    box = None
+    if ops_ and ops_[-1][0] == "crop":
+        ops_, box = ops_[:-1], ops_[-1][1]
+    if im is None and ops_:                    # a blank cell stays black through any resize
+        ops_ = ()
+    for op in ops_:
+        im = resample.resize(im, op[1], op[2]) if op[0] == "resize" else resample.crop(im, op[1])
+    w, h = cell.size
+    ops.u8_to_model_input(im, box or (0, 0, w, h), out, col0)
 
 
 def _load_file(path: str, device) -> dict:
@@ -207,42 +292,36 @@ class VisualClozeModel:
     # ------------------------------------------------------------------------------------------------
     def _prepare_grid(self, images):
         """Resize / crop every cell to its row's reference size; blank + mask for the missing targets of the last row
-        (visualcloze.py:300-360)."""
-        grid_h, grid_w, resolution = self.grid_h, self.grid_w, self.resolution
-        processed, mask_position = [], []
-        target_size = upsampling_size = None
-        for i in range(grid_h):
-            reference_size = None
-            for j in range(grid_w):
-                if images[i][j] is not None:
-                    if i == grid_h - 1 and upsampling_size is None:
-                        upsampling_size = images[i][j].size
-                    reference_size = resize_with_aspect_ratio(images[i][j], resolution).size
-                    if i == grid_h - 1 and target_size is None:
-                        target_size = reference_size
-                    break
-            for j in range(grid_w):
-                if images[i][j] is not None:
-                    t = resize_with_aspect_ratio(images[i][j], resolution)
-                    if t.width <= t.height:
-                        t = t.resize((reference_size[0], int(reference_size[0] / t.width * t.height)))
-                    else:
-                        t = t.resize((int(reference_size[1] / t.height * t.width), reference_size[1]))
-                    processed.append(center_crop(t, reference_size))
-                    if i == grid_h - 1:
-                        mask_position.append(0)
-                else:
-                    if i != grid_h - 1:
-                        raise ValueError("Please provide each image in the in-context example.")
-                    processed.append(Image.new("RGB", reference_size or (resolution, resolution), (0, 0, 0)))
-                    mask_position.append(1)
-        if len(mask_position) > 1 and sum(mask_position) > 1:
-            new_w = 384 if target_size is None else target_size[0]
-            for k, im in enumerate(processed):
-                new_h = int(im.height * (new_w / im.width))
-                new_w, new_h = int(new_w / 16) * 16, int(new_h / 16) * 16
-                processed[k] = im.resize((new_w, new_h))
+        (visualcloze.py:300-360), with Pillow on the host.  -> (cells as PIL images, mask_position, upsampling_size)."""
+        sizes = [[None if im is None else im.size for im in row] for row in images]
+        cells, mask_position, upsampling_size = grid_plan(sizes, self.grid_h, self.grid_w, self.resolution)
+        processed = [run_cell_pil(images[k // self.grid_w][k % self.grid_w], c) for k, c in enumerate(cells)]
         return processed, mask_position, upsampling_size
+
+    def _grid_rows(self, images):
+        """The model input of every grid row built on the device, bit-identical to ``torch.cat([image_transform(c) for c in
+        row], dim=2)`` over the cells of ``_prepare_grid``: each RGB image is uploaded once, resampled by libvcb200's Pillow
+        resampler and written straight into its row.  -> (rows: fp32 [3, h, W] on the device, mask_position, upsampling_size)."""
+        grid_h, grid_w = self.grid_h, self.grid_w
+        sizes = [[None if im is None else im.size for im in row] for row in images]
+        cells, mask_position, upsampling_size = grid_plan(sizes, grid_h, grid_w, self.resolution)
+        rows = []
+        for i in range(grid_h):
+            plans = cells[i * grid_w:(i + 1) * grid_w]
+            widths = [c.size[0] for c in plans]
+            row = torch.empty(3, plans[0].size[1], sum(widths), dtype=torch.float32, device=self.device)
+            col = 0
+            for j, cell in enumerate(plans):
+                image = None if images[i][j] is None else resample.upload(images[i][j], self.device)
+                run_cell_device(image, cell, row, col)
+                col += widths[j]
+            rows.append(row)
+        return rows, mask_position, upsampling_size
+
+    def _sdedit_resize(self, tile: torch.Tensor, box, size) -> torch.Tensor:
+        """The SDEdit input image: the ``box`` crop of a uint8 [H, W, 3] device image, resized with BICUBIC to ``size``, on
+        the device (``image.crop(box).resize(size)``)."""
+        return resample.resize(resample.crop(tile, box), size, resample.BICUBIC)
 
     @torch.no_grad()
     def process_images(self, images, prompts, seed: int = 0, cfg: int = 30, steps: int = 30, upsampling_steps: int = 10,
@@ -253,15 +332,13 @@ class VisualClozeModel:
         grid_h, grid_w = self.grid_h, self.grid_w
         for i in range(grid_h):
             images[i] = [im.convert("RGB") if im is not None else None for im in images[i]]
-        processed, mask_position, upsampling_size = self._prepare_grid(images)
+        rows, mask_position, upsampling_size = self._grid_rows(images)
 
         dev, dt = self.device, self.dtype
-        rows, fill_mask = [], []
-        for i in range(grid_h):
-            cells = [self.image_transform(im) for im in processed[i * grid_w:(i + 1) * grid_w]]
-            h, w = cells[0].shape[1], cells[0].shape[2]
+        fill_mask = []
+        for i, r in enumerate(rows):
+            h, w = r.shape[1], r.shape[2] // grid_w
             marks = mask_position if i == grid_h - 1 else [0] * grid_w
-            rows.append(torch.cat(cells, dim=2).to(dev))
             fill_mask.append(torch.cat([torch.full((1, 1, h, w), float(m), device=dev) for m in marks], dim=3))
         fill_cond = torch.cat([self._encode_tokens(r) for r in rows], dim=1)
         fill_mask = torch.cat([_pack_mask(m) for m in fill_mask], dim=1).to(dt)
@@ -284,25 +361,34 @@ class VisualClozeModel:
         n_tok = qh * qw // 256
         start = sum(h * w // 256 for h, w in sizes[:-1])
         tile = self.ae.decode_packed(samples[:, start:start + n_tok, :], qh // 16, qw // 16)[0]     # uint8 [3, H, W]
-        query = Image.fromarray(tile.permute(1, 2, 0).cpu().numpy())
+        tile = tile.permute(1, 2, 0).contiguous()                                                      # uint8 [H, W, 3]
+        query = None if is_upsampling else Image.fromarray(tile.cpu().numpy())
         torch.cuda.empty_cache()
 
         ret = []
-        ret_w, ret_h = query.width, query.height
+        ret_h, ret_w = tile.shape[0], tile.shape[1]
         for j in range(grid_w):
             if not mask_position[j]:
                 continue
-            cropped = query.crop((j * ret_w // grid_w, 0, (j + 1) * ret_w // grid_w, ret_h))
+            box = (j * ret_w // grid_w, 0, (j + 1) * ret_w // grid_w, ret_h)
             if is_upsampling:
-                cropped = self.upsampling(cropped, upsampling_size, cfg, upsampling_steps=upsampling_steps,
-                                          upsampling_noise=upsampling_noise, generator=rng, content_prompt=prompts[2])
-            ret.append(cropped)
+                ret.append(self._upsampling(tile, box, upsampling_size, cfg, upsampling_steps, upsampling_noise, rng, prompts[2]))
+            else:
+                ret.append(query.crop(box))
         return ret
 
     @torch.no_grad()
     def upsampling(self, image, target_size, cfg, upsampling_steps, upsampling_noise, generator, content_prompt):
         """SDEdit second stage (visualcloze.py:147-245): noise the resized image to `upsampling_noise`, denoise with an
-        all-ones fill mask over a blank condition, 1x1 grid."""
+        all-ones fill mask over a blank condition, 1x1 grid.  ``image`` (PIL; a mode other than RGB is converted as
+        ``image_transform`` converts it) is uploaded once; the resize and the model input are made on the device."""
+        if image.mode != "RGB":
+            image = to_rgb_if_rgba(image).convert("RGB")
+        return self._upsampling(resample.upload(image, self.device), (0, 0, image.width, image.height), target_size, cfg,
+                                upsampling_steps, upsampling_noise, generator, content_prompt)
+
+    def _upsampling(self, tile, box, target_size, cfg, upsampling_steps, upsampling_noise, generator, content_prompt):
+        """``upsampling`` of the ``box`` crop of a uint8 [H, W, 3] device image."""
         for c in _CONTENT_PREFIXES:
             if content_prompt.startswith(c):
                 content_prompt = content_prompt.replace(c, "")
@@ -312,12 +398,13 @@ class VisualClozeModel:
             ar = target_size[0] / target_size[1]
             new_h = int((1024 * 1024 / ar) ** 0.5)
             target_size = (int(new_h * ar), new_h)
-        image = image.resize(((target_size[0] // 16) * 16, (target_size[1] // 16) * 16))
+        size = ((target_size[0] // 16) * 16, (target_size[1] // 16) * 16)
+        image = self._sdedit_resize(tile, box, size)
         if upsampling_noise >= 1.0:
-            return image
+            return Image.fromarray(image.cpu().numpy())
         self.sample_fn = self._make_sample_fn(int(upsampling_steps), False, 1.0, upsampling_noise)
         dev, dt = self.device, self.dtype
-        x = self.image_transform(image).to(dev)
+        x = ops.u8_to_model_input(image, (0, 0) + size, torch.empty(3, size[1], size[0], dtype=torch.float32, device=dev), 0)
         latent = self._encode_tokens(x)
         blank = self._encode_tokens(torch.zeros_like(x))
         lh, lw = x.shape[1] // 8, x.shape[2] // 8
