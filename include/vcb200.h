@@ -379,6 +379,17 @@ int vcb_flux_set_first_block_cache(vcb_flux* f, float threshold);
 /* evaluations computed / skipped since the last vcb_flux_prepare, and diff of the latest one (+inf for the first evaluation after
  * prepare, which has nothing to compare with; NaN before any) */
 int vcb_flux_cache_stats(const vcb_flux* f, int32_t* computed, int32_t* skipped, float* last_diff);
+/* vcb_flux_set_first_block_cache with a choice of decision mode: per_sample 0 is vcb_flux_set_first_block_cache (one decision per
+ * batch, bitwise unchanged); 1 decides every sample on its own valid img rows, so a sample's decisions do not depend on the other
+ * samples it shares the batch with (at B = 1 both modes are bitwise equal).  Per evaluation: every sample skips -> the skip path
+ * above; none skips -> a computed evaluation as above; mixed -> the blocks run for the whole batch, then the img rows of each
+ * skipped sample become bf16(x1 + R) with its own x1 and R, and r_ref / R are updated for the computed samples only.  In this mode
+ * vcb_flux_cache_stats counts an evaluation as skipped when every sample skipped (computed otherwise) and reports the largest
+ * sample diff.  Takes at most 1024 samples.  Changing the mode while the cache is on asks for a new vcb_flux_prepare. */
+int vcb_flux_set_first_block_cache_ex(vcb_flux* f, float threshold, int32_t per_sample);
+/* per-sample counters since the last vcb_flux_prepare: computed[b] / skipped[b] evaluations and last_diff[b] of sample b (B = the
+ * prepared batch).  In per-batch mode every sample gets the batch's values of vcb_flux_cache_stats. */
+int vcb_flux_cache_stats_per_sample(const vcb_flux* f, int32_t B, int32_t* computed, int32_t* skipped, float* last_diff);
 
 /* ---- single-image sequence parallelism over NVLink peer memory (SURVEY.md 8f-2: the reference has no multi-GPU
  * inference; the join point is the attention call, layers.py:177-187 / 236-241) -----------------------------------

@@ -213,6 +213,8 @@ _OPTIONAL: dict = {
     "vcb_flux_forward": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]),
     "vcb_flux_set_first_block_cache": (C.c_int, [C.c_void_p, C.c_float]),
     "vcb_flux_cache_stats": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_float)]),
+    "vcb_flux_set_first_block_cache_ex": (C.c_int, [C.c_void_p, C.c_float, C.c_int32]),
+    "vcb_flux_cache_stats_per_sample": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_float)]),
     # sequence-parallel single-image mode
     "vcb_attention_fwd_sp": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                        C.POINTER(C.c_void_p), C.c_int32, C.c_int32, C.c_int64, C.c_int32, C.c_void_p]),

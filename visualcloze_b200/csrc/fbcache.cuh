@@ -1,9 +1,10 @@
 // fbcache.cuh -- kernels of the opt-in first-block cache of the FLUX-DiT engine (vcb_flux_set_first_block_cache).
 //
 // After double block 0 the engine compares the img-row residual of that block, r_k = bf16(x1 - x0), with the one of the last
-// computed evaluation, r_ref: diff = sum|r_k - r_ref| / sum|r_ref| over the valid img rows of every sample (one decision per
-// batch).  A skipped evaluation then writes x = bf16(x1 + R), R = x_final - x1 (fp32) of the last computed evaluation, and goes
-// straight to the final layer.  Buffers are [B * Li, H] (row r = b * Li + i); x itself is the joint [B, L, H] residual stream.
+// computed evaluation, r_ref: diff = sum|r_k - r_ref| / sum|r_ref| over the valid img rows of every sample of a decision group
+// (per-batch mode: one group, the whole batch; per-sample mode: one group per sample).  A skipped evaluation then writes
+// x = bf16(x1 + R), R = x_final - x1 (fp32) of the last computed evaluation, and goes straight to the final layer.  Buffers are
+// [B * Li, H] (row r = b * Li + i); x itself is the joint [B, L, H] residual stream.
 #pragma once
 #include <cuda_bf16.h>
 
@@ -16,6 +17,7 @@ namespace vcb {
 constexpr int kFbcWarps = 8;            // one warp per img row, 8 rows per CTA
 constexpr int kFbcMaxBlocks = 1024;     // CTAs of the partial-sum pass = number of partial-sum slots
 constexpr int kFbcThreads = 256;        // elementwise residual kernels
+constexpr int kFbcDecideWarps = 8;      // decision kernel: one warp per group, groups strided over the warps
 
 struct FbcRows {
     int B, Li, Lt, L, H;
@@ -34,15 +36,19 @@ __device__ __forceinline__ int64_t fbc_x_row(const FbcRows& g, int r) {
 }
 
 // Pass 1.  Every row: r_k = bf16(x1 - x0) overwrites the x0 copy.  Valid rows (not when `first`: there is no r_ref yet): each CTA
-// sums num = sum|r_k - r_ref| and den = sum|r_ref| in fp32 into its slot part[blockIdx.x].  Fixed order -- a lane walks its
-// columns row by row, the lanes of a warp combine by a butterfly, the warps in index order -- so equal inputs give equal sums.
+// sums num = sum|r_k - r_ref| and den = sum|r_ref| in fp32 into its slot part[blockIdx.x].  The grid is `groups` equal runs of
+// CTAs, run k covering the rows of group k only (groups = 1: every row; groups = B: sample k), so no slot straddles two groups.
+// Fixed order -- a lane walks its columns row by row, the lanes of a warp combine by a butterfly, the warps in index order -- so
+// equal inputs give equal sums, and one group of nb CTAs sums exactly as the per-batch pass of nb CTAs does.
 __global__ void __launch_bounds__(kFbcWarps * 32) fbc_partial_kernel(__nv_bfloat16* __restrict__ x0_rk, const __nv_bfloat16* __restrict__ x,
                                                                      const __nv_bfloat16* __restrict__ r_ref, FbcRows g, int first,
-                                                                     float2* __restrict__ part) {
+                                                                     int groups, float2* __restrict__ part) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int rows = g.B * g.Li, nv = g.H / 8;
+    const int nbs = gridDim.x / groups, grp = blockIdx.x / nbs, blk = blockIdx.x - grp * nbs;
+    const int rows = g.B * g.Li / groups, r0 = grp * rows, nv = g.H / 8;
     float num = 0.f, den = 0.f;
-    for (int r = blockIdx.x * kFbcWarps + warp; r < rows; r += gridDim.x * kFbcWarps) {
+    for (int k = blk * kFbcWarps + warp; k < rows; k += nbs * kFbcWarps) {
+        const int r = r0 + k;
         const bool count = !first && (r % g.Li) < fbc_valid_rows(g, r / g.Li);
         uint4* a = reinterpret_cast<uint4*>(x0_rk + (int64_t)r * g.H);
         const uint4* c = reinterpret_cast<const uint4*>(x + fbc_x_row(g, r) * g.H);
@@ -85,21 +91,33 @@ __global__ void __launch_bounds__(kFbcWarps * 32) fbc_partial_kernel(__nv_bfloat
     }
 }
 
-// Pass 2, one warp: the n slots in a fixed order -> out = {num, den, diff, skip}; diff = num / den (+inf when `first`), skip =
-// !first && diff < threshold (a NaN diff -- no residual to compare with -- computes).
-__global__ void __launch_bounds__(32) fbc_decide_kernel(const float2* __restrict__ part, int n, float threshold, int first,
-                                                        float* __restrict__ out) {
-    float num = 0.f, den = 0.f;
-    for (int k = threadIdx.x; k < n; k += 32) { num += part[k].x; den += part[k].y; }
+// Pass 2: warp w decides groups w, w + warps, ...; group k sums its nbs slots in a fixed order -> out[4k..4k+3] = {num, den, diff,
+// skip}; diff = num / den (+inf when `first`), skip = !first && diff < threshold (a NaN diff -- no residual to compare with --
+// computes).  out[4 * groups] = the number of groups that skip (groups = all skipped, 0 = none).
+__global__ void __launch_bounds__(kFbcDecideWarps * 32) fbc_decide_kernel(const float2* __restrict__ part, int nbs, int groups,
+                                                                          float threshold, int first, float* __restrict__ out) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int grp = warp; grp < groups; grp += blockDim.x >> 5) {
+        const float2* p = part + grp * nbs;
+        float num = 0.f, den = 0.f;
+        for (int k = lane; k < nbs; k += 32) { num += p[k].x; den += p[k].y; }
 #pragma unroll
-    for (int o = 16; o; o >>= 1) {
-        num += __shfl_xor_sync(0xffffffffu, num, o);
-        den += __shfl_xor_sync(0xffffffffu, den, o);
+        for (int o = 16; o; o >>= 1) {
+            num += __shfl_xor_sync(0xffffffffu, num, o);
+            den += __shfl_xor_sync(0xffffffffu, den, o);
+        }
+        if (lane == 0) {
+            const float diff = first ? INFINITY : num / den;
+            float* o = out + 4 * grp;
+            o[0] = num; o[1] = den; o[2] = diff;
+            o[3] = (!first && diff < threshold) ? 1.f : 0.f;
+        }
     }
+    __syncthreads();
     if (threadIdx.x == 0) {
-        const float diff = first ? INFINITY : num / den;
-        out[0] = num; out[1] = den; out[2] = diff;
-        out[3] = (!first && diff < threshold) ? 1.f : 0.f;
+        int n = 0;
+        for (int k = 0; k < groups; ++k) n += out[4 * k + 3] != 0.f;
+        out[4 * groups] = (float)n;
     }
 }
 
@@ -148,23 +166,25 @@ __global__ void __launch_bounds__(kFbcThreads) fbc_apply_residual_kernel(__nv_bf
     }
 }
 
-inline int fbc_partial_blocks(const FbcRows& g) {
-    const int need = (g.B * g.Li + kFbcWarps - 1) / kFbcWarps;
-    return need < kFbcMaxBlocks ? need : kFbcMaxBlocks;
+// CTAs of one group's partial-sum run: enough for one warp per row, at most kFbcMaxBlocks over all groups
+inline int fbc_group_blocks(const FbcRows& g, int groups) {
+    const int need = (g.B * g.Li / groups + kFbcWarps - 1) / kFbcWarps, cap = kFbcMaxBlocks / groups;
+    return need < cap ? need : cap;
 }
 
-// both passes of the decision; `res` [4] fp32 device, `part` [kFbcMaxBlocks] float2 device
-inline int fbc_decide(uint16_t* x0_rk, const uint16_t* x, const uint16_t* r_ref, const FbcRows& g, bool first, float threshold,
+// both passes of the decision for `groups` (1 or B) groups; `res` [4 * groups + 1] fp32 device, `part` [kFbcMaxBlocks] float2 device
+inline int fbc_decide(uint16_t* x0_rk, const uint16_t* x, const uint16_t* r_ref, const FbcRows& g, int groups, bool first, float threshold,
                       float2* part, float* res, cudaStream_t st) {
-    const int nb = fbc_partial_blocks(g);
+    const int nbs = fbc_group_blocks(g, groups);
     {
         ProfScope prof(PROF_OTHER, st);
-        fbc_partial_kernel<<<nb, kFbcWarps * 32, 0, st>>>(reinterpret_cast<__nv_bfloat16*>(x0_rk), reinterpret_cast<const __nv_bfloat16*>(x),
-                                                          reinterpret_cast<const __nv_bfloat16*>(r_ref), g, first ? 1 : 0, part);
+        fbc_partial_kernel<<<nbs * groups, kFbcWarps * 32, 0, st>>>(reinterpret_cast<__nv_bfloat16*>(x0_rk), reinterpret_cast<const __nv_bfloat16*>(x),
+                                                                    reinterpret_cast<const __nv_bfloat16*>(r_ref), g, first ? 1 : 0, groups, part);
         if (int rc = check_launch("fbc_partial")) return rc;
     }
     ProfScope prof(PROF_OTHER, st);
-    fbc_decide_kernel<<<1, 32, 0, st>>>(part, nb, threshold, first ? 1 : 0, res);
+    const int warps = groups < kFbcDecideWarps ? groups : kFbcDecideWarps;
+    fbc_decide_kernel<<<1, warps * 32, 0, st>>>(part, nbs, groups, threshold, first ? 1 : 0, res);
     return check_launch("fbc_decide");
 }
 

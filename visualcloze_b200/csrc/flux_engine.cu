@@ -51,18 +51,24 @@ struct vcb_flux {
     // T [max(B * L, E * B), lora_rmax] bf16, written by each LoRA Linear's down-projection and read by its k-tail right after
     int lora_rmax = 0;
     uint16_t* lora_t = nullptr;
-    // first-block cache (vcb_flux_set_first_block_cache; threshold 0 = off).  fbc_buf[fbc_ref] holds r_ref, the block-0 residual
-    // of the last computed evaluation; the other one takes the x0 copy, which the decision turns into r_k in place -- a computed
-    // evaluation then swaps the two and parks x1 in the freed one until the residual R is stored
+    // first-block cache (vcb_flux_set_first_block_cache_ex; threshold 0 = off).  fbc_buf[fbc_ref] holds r_ref, the block-0
+    // residual of the last computed evaluation; the other one takes the x0 copy, which the decision turns into r_k in place -- an
+    // evaluation computed for every sample then swaps the two and parks x1 in the freed one until the residual R is stored.  When
+    // only some samples compute (per-sample mode), their rows of r_k are copied into r_ref instead and x1 overwrites r_k.
     float fbc_threshold = 0.f;
+    bool fbc_per_sample = false;      // one decision per sample instead of one per batch
     uint16_t* fbc_buf[2] = {};        // [B * Li, H] bf16 each
     int fbc_ref = 0;
-    float* fbc_R = nullptr;           // [B * Li, H] fp32: x_final - x1 of the last computed evaluation
+    float* fbc_R = nullptr;           // [B * Li, H] fp32: x_final - x1 of the last computed evaluation (per sample)
     float2* fbc_part = nullptr;       // [kFbcMaxBlocks] partial sums of the decision
-    float* fbc_res = nullptr;         // [4] num, den, diff, skip (device)
-    float* fbc_host = nullptr;        // [4] pinned copy read by the host
+    float* fbc_res = nullptr;         // [4 * groups + 1] per group num, den, diff, skip; then the number of skipping groups (device)
+    float* fbc_host = nullptr;        // pinned copy of fbc_res read by the host
+    int fbc_host_cap = 0;             // floats fbc_host holds
     int32_t fbc_computed = 0, fbc_skipped = 0;
     float fbc_last_diff = NAN;
+    std::vector<int32_t> fbc_s_computed, fbc_s_skipped;    // [B] per-sample counters (per-sample mode)
+    std::vector<float> fbc_s_diff;                         // [B] latest per-sample diff
+    std::vector<char> fbc_s_skip;                          // [B] this evaluation's per-sample decision
     ~vcb_flux() { if (fbc_host) cudaFreeHost(fbc_host); }
 };
 
@@ -111,7 +117,7 @@ int64_t carve(vcb_flux* f, uint8_t* base, int B, int Li, int Lt, int E) {
     uint16_t* fbc_b1 = cv.take<uint16_t>(fbc_n);
     float* fbc_R = cv.take<float>(fbc_n);
     float2* fbc_part = cv.take<float2>(fbc_n ? kFbcMaxBlocks : 0);
-    float* fbc_res = cv.take<float>(fbc_n ? 4 : 0);
+    float* fbc_res = cv.take<float>(fbc_n ? 4 * (f->fbc_per_sample ? B : 1) + 1 : 0);
     // sequence-parallel: qkv [W*L, 3H/W] and cat [L, H+mlp] are the caller's peer-mapped allocations (same sizes)
     const bool sp = f->sp_world > 1;
     uint16_t* qkv = sp ? static_cast<uint16_t*>(f->sp_qkv[f->sp_rank]) : cv.take<uint16_t>((int64_t)B * L * 3 * H);
@@ -238,21 +244,39 @@ extern "C" int vcb_flux_set_fp8(vcb_flux* f, int32_t level) {
     return 0;
 }
 
-extern "C" int vcb_flux_set_first_block_cache(vcb_flux* f, float threshold) {
+extern "C" int vcb_flux_set_first_block_cache_ex(vcb_flux* f, float threshold, int32_t per_sample) {
     if (!f) return set_error("flux_set_first_block_cache: null engine");
     if (!std::isfinite(threshold) || threshold < 0.f) return set_error("flux_set_first_block_cache: threshold must be a finite number >= 0 (0 = off)");
+    if (per_sample != 0 && per_sample != 1) return set_error("flux_set_first_block_cache: per_sample must be 0 (one decision per batch) or 1");
     if (threshold > 0.f) {
         if (f->sp_world > 1) return set_error("flux_set_first_block_cache: the skip decision would have to agree across the sequence-parallel ranks");
         if (f->cfg.depth < 1) return set_error("flux_set_first_block_cache: the cache decides after the first double block (depth >= 1)");
     }
-    if ((threshold > 0.f) != (f->fbc_threshold > 0.f)) f->prepared = false;    // the workspace layout depends on it
+    // the workspace layout depends on whether the cache is on and, while on, on the mode
+    if ((threshold > 0.f) != (f->fbc_threshold > 0.f) || (threshold > 0.f && (per_sample != 0) != f->fbc_per_sample)) f->prepared = false;
     f->fbc_threshold = threshold;
+    f->fbc_per_sample = per_sample != 0;
     return 0;
 }
+
+extern "C" int vcb_flux_set_first_block_cache(vcb_flux* f, float threshold) { return vcb_flux_set_first_block_cache_ex(f, threshold, 0); }
 
 extern "C" int vcb_flux_cache_stats(const vcb_flux* f, int32_t* computed, int32_t* skipped, float* last_diff) {
     if (!f || !computed || !skipped || !last_diff) return set_error("flux_cache_stats: null argument");
     *computed = f->fbc_computed; *skipped = f->fbc_skipped; *last_diff = f->fbc_last_diff;
+    return 0;
+}
+
+extern "C" int vcb_flux_cache_stats_per_sample(const vcb_flux* f, int32_t B, int32_t* computed, int32_t* skipped, float* last_diff) {
+    if (!f || !computed || !skipped || !last_diff) return set_error("flux_cache_stats_per_sample: null argument");
+    if (!f->prepared) return set_error("flux_cache_stats_per_sample: call vcb_flux_prepare first");
+    if (B != f->B) return set_error("flux_cache_stats_per_sample: B (%d) must be the prepared batch (%d)", B, f->B);
+    const bool own = f->fbc_per_sample && f->fbc_threshold > 0.f;
+    for (int b = 0; b < B; ++b) {          // per-batch mode: every sample shares the batch's decisions
+        computed[b] = own ? f->fbc_s_computed[b] : f->fbc_computed;
+        skipped[b] = own ? f->fbc_s_skipped[b] : f->fbc_skipped;
+        last_diff[b] = own ? f->fbc_s_diff[b] : f->fbc_last_diff;
+    }
     return 0;
 }
 
@@ -313,9 +337,17 @@ extern "C" int vcb_flux_prepare(vcb_flux* f, void* workspace, int64_t workspace_
     f->B = B; f->Li = Li; f->Lt = Lt; f->L = Li + Lt; f->E = n_evals; f->seqlens = seqlens;
     f->prepared = false;
     f->fbc_ref = 0; f->fbc_computed = 0; f->fbc_skipped = 0; f->fbc_last_diff = NAN;
-    if (f->fbc_threshold > 0.f && !f->fbc_host) {       // where vcb_flux_forward reads the cache's decision
-        cudaError_t e = cudaMallocHost(reinterpret_cast<void**>(&f->fbc_host), 4 * sizeof(float));
-        if (e != cudaSuccess) { f->fbc_host = nullptr; return set_error("flux_prepare: pinned memory: %s", cudaGetErrorString(e)); }
+    f->fbc_s_computed.assign(B, 0); f->fbc_s_skipped.assign(B, 0); f->fbc_s_diff.assign(B, NAN); f->fbc_s_skip.assign(B, 0);
+    if (f->fbc_threshold > 0.f) {
+        const int groups = f->fbc_per_sample ? B : 1;
+        if (groups > kFbcMaxBlocks) return set_error("flux_prepare: the per-sample first-block cache takes at most %d samples", kFbcMaxBlocks);
+        if (f->fbc_host_cap < 4 * groups + 1) {         // where vcb_flux_forward reads the cache's decision
+            if (f->fbc_host) cudaFreeHost(f->fbc_host);
+            f->fbc_host = nullptr; f->fbc_host_cap = 0;
+            cudaError_t e = cudaMallocHost(reinterpret_cast<void**>(&f->fbc_host), (4 * groups + 1) * sizeof(float));
+            if (e != cudaSuccess) { f->fbc_host = nullptr; return set_error("flux_prepare: pinned memory: %s", cudaGetErrorString(e)); }
+            f->fbc_host_cap = 4 * groups + 1;
+        }
     }
     const int H = c.hidden, EB = n_evals * B;
     int rc;
@@ -465,31 +497,75 @@ int adaln(const vcb_flux* f, const StreamView& sv0, const uint16_t* shift0, cons
 FbcRows fbc_rows(const vcb_flux* f) { return FbcRows{f->B, f->Li, f->Lt, f->L, f->cfg.hidden, f->seqlens}; }
 
 // First-block cache, right after double block 0: decide (one stream wait, except on the first evaluation since prepare, which is
-// always computed), then either write x = bf16(x1 + R) (skip) or make r_k the new r_ref and keep x1 for the residual R.
-int fbc_after_first_block(vcb_flux* f, cudaStream_t st, bool* skip) {
+// always computed), then either write x = bf16(x1 + R) (every group skips) or make r_k the new r_ref and keep x1 for the residual R
+// (every group computes).  Per-sample mode with mixed decisions (*mixed): the blocks run for the whole batch; the computed samples'
+// rows of r_k become their r_ref, and x1 of every sample is kept for fbc_finish.
+int fbc_after_first_block(vcb_flux* f, cudaStream_t st, bool* skip, bool* mixed) {
     const bool first = f->fbc_computed == 0 && f->fbc_skipped == 0;
     const FbcRows g = fbc_rows(f);
+    const int groups = f->fbc_per_sample ? f->B : 1;
     uint16_t* x0_rk = f->fbc_buf[f->fbc_ref ^ 1];
-    if (int rc = fbc_decide(x0_rk, f->x, f->fbc_buf[f->fbc_ref], g, first, f->fbc_threshold, f->fbc_part, f->fbc_res, st)) return rc;
-    *skip = false;
+    if (int rc = fbc_decide(x0_rk, f->x, f->fbc_buf[f->fbc_ref], g, groups, first, f->fbc_threshold, f->fbc_part, f->fbc_res, st)) return rc;
+    *skip = *mixed = false;
     f->fbc_last_diff = INFINITY;
+    int n_skip = 0;
     if (!first) {
-        cudaError_t e = cudaMemcpyAsync(f->fbc_host, f->fbc_res, 4 * sizeof(float), cudaMemcpyDeviceToHost, st);
+        cudaError_t e = cudaMemcpyAsync(f->fbc_host, f->fbc_res, (4 * groups + 1) * sizeof(float), cudaMemcpyDeviceToHost, st);
         if (e == cudaSuccess) e = cudaStreamSynchronize(st);
         if (e != cudaSuccess) return set_error("flux_forward: first-block cache decision: %s", cudaGetErrorString(e));
-        *skip = f->fbc_host[3] != 0.f;
+        n_skip = (int)f->fbc_host[4 * groups];
         f->fbc_last_diff = f->fbc_host[2];
     }
-    if (*skip) {
+    if (f->fbc_per_sample) {
+        for (int b = 0; b < f->B; ++b) {
+            const bool sb = !first && f->fbc_host[4 * b + 3] != 0.f;
+            f->fbc_s_skip[b] = sb;
+            f->fbc_s_diff[b] = first ? INFINITY : f->fbc_host[4 * b + 2];
+            ++(sb ? f->fbc_s_skipped[b] : f->fbc_s_computed[b]);
+            if (b == 0 || f->fbc_s_diff[b] > f->fbc_last_diff) f->fbc_last_diff = f->fbc_s_diff[b];   // the largest sample diff
+        }
+    }
+    const int64_t H = f->cfg.hidden, img_bytes = (int64_t)f->Li * H * 2;
+    if (n_skip == groups) {
+        *skip = true;
         ++f->fbc_skipped;
         return fbc_apply_residual(f->x, f->fbc_R, g, st);
     }
     ++f->fbc_computed;
-    f->fbc_ref ^= 1;                                   // r_k is the reference of the next decisions
-    const int64_t H = f->cfg.hidden;
-    cudaError_t e = cudaMemcpy2DAsync(f->fbc_buf[f->fbc_ref ^ 1], (size_t)f->Li * H * 2, f->x + (int64_t)f->Lt * H, (size_t)f->L * H * 2,
-                                      (size_t)f->Li * H * 2, f->B, cudaMemcpyDeviceToDevice, st);
+    if (n_skip == 0) {
+        f->fbc_ref ^= 1;                               // r_k is the reference of the next decisions
+    } else {
+        *mixed = true;
+        for (int b = 0; b < f->B; ++b) {
+            if (f->fbc_s_skip[b]) continue;
+            cudaError_t e = cudaMemcpyAsync(f->fbc_buf[f->fbc_ref] + b * (int64_t)f->Li * H, x0_rk + b * (int64_t)f->Li * H, (size_t)img_bytes,
+                                            cudaMemcpyDeviceToDevice, st);
+            if (e != cudaSuccess) return set_error("flux_forward: first-block cache r_ref copy: %s", cudaGetErrorString(e));
+        }
+    }
+    cudaError_t e = cudaMemcpy2DAsync(f->fbc_buf[f->fbc_ref ^ 1], (size_t)img_bytes, f->x + (int64_t)f->Lt * H, (size_t)f->L * H * 2,
+                                      (size_t)img_bytes, f->B, cudaMemcpyDeviceToDevice, st);
     if (e != cudaSuccess) return set_error("flux_forward: first-block cache x1 copy: %s", cudaGetErrorString(e));
+    return 0;
+}
+
+// First-block cache, after the last block of a computed evaluation: R = x_final - x1 for the computed samples; with mixed decisions
+// the img rows of each skipped sample become bf16(x1 + R) with its own x1 and R (the same arithmetic as a skipped evaluation)
+int fbc_finish(vcb_flux* f, bool mixed, cudaStream_t st) {
+    const uint16_t* x1c = f->fbc_buf[f->fbc_ref ^ 1];
+    if (!mixed) return fbc_store_residual(f->x, x1c, f->fbc_R, fbc_rows(f), st);
+    const int64_t H = f->cfg.hidden, n = (int64_t)f->Li * H;
+    const FbcRows one{1, f->Li, f->Lt, f->L, f->cfg.hidden, nullptr};
+    for (int b = 0; b < f->B; ++b) {
+        uint16_t* xb = f->x + (int64_t)b * f->L * H;
+        if (!f->fbc_s_skip[b]) {
+            if (int rc = fbc_store_residual(xb, x1c + b * n, f->fbc_R + b * n, one, st)) return rc;
+            continue;
+        }
+        cudaError_t e = cudaMemcpyAsync(xb + (int64_t)f->Lt * H, x1c + b * n, (size_t)n * 2, cudaMemcpyDeviceToDevice, st);
+        if (e != cudaSuccess) return set_error("flux_forward: first-block cache x1 restore: %s", cudaGetErrorString(e));
+        if (int rc = fbc_apply_residual(xb, f->fbc_R + b * n, one, st)) return rc;
+    }
     return 0;
 }
 
@@ -524,7 +600,7 @@ extern "C" int vcb_flux_forward(vcb_flux* f, int32_t e, const void* img, int64_t
     }
     f->stats_valid = false;                  // x was just (re)written by img_in and the txt copy: no statistics yet
     const bool fbc = f->fbc_threshold > 0.f;
-    bool skip = false;
+    bool skip = false, mixed = false;
     if (fbc) {                               // x0: the img rows as img_in left them
         cudaError_t ce = cudaMemcpy2DAsync(f->fbc_buf[f->fbc_ref ^ 1], (size_t)Li * H * 2, f->x + (int64_t)Lt * H, (size_t)L * H * 2,
                                            (size_t)Li * H * 2, B, cudaMemcpyDeviceToDevice, st);
@@ -578,7 +654,7 @@ extern "C" int vcb_flux_forward(vcb_flux* f, int32_t e, const void* img, int64_t
             f->stats_valid = true;
         }
         if (i == 0 && fbc) {
-            if ((rc = fbc_after_first_block(f, st, &skip))) return rc;
+            if ((rc = fbc_after_first_block(f, st, &skip, &mixed))) return rc;
             if (skip) break;
         }
     }
@@ -596,7 +672,7 @@ extern "C" int vcb_flux_forward(vcb_flux* f, int32_t e, const void* img, int64_t
         f->stats_valid = true;
     }
     if (fbc) {
-        if (!skip && (rc = fbc_store_residual(f->x, f->fbc_buf[f->fbc_ref ^ 1], f->fbc_R, fbc_rows(f), st))) return rc;
+        if (!skip && (rc = fbc_finish(f, mixed, st))) return rc;
         // the final LayerNorm computes its own statistics whenever the cache is on: a skipped evaluation (whose x no GEMM
         // epilogue wrote) and a computed one then share the arithmetic, so equal residual streams give equal outputs
         f->stats_valid = false;

@@ -66,6 +66,7 @@ class FluxEngine:
         self._shape = None
         self._sp = None
         self._fbc = 0.0
+        self._fbc_per_sample = False
         self._freqs = _freqs().to(self.device)
 
     # ---- single-image sequence parallelism (SURVEY.md 8f-2) -------------------------------------------
@@ -85,17 +86,19 @@ class FluxEngine:
         self._shape = None
 
     # ---- first-block cache (vcb_flux_set_first_block_cache) ------------------------------------------
-    def set_first_block_cache(self, threshold) -> None:
+    def set_first_block_cache(self, threshold, per_sample: bool = False) -> None:
         """``threshold`` > 0: an evaluation whose double-block-0 residual moved by less than ``threshold`` (relative L1) since the
-        last computed evaluation reuses that evaluation's residual of the remaining blocks; 0 / None: off.  Each ``forward`` then
-        waits for its decision on the host (not capturable in a CUDA graph)."""
+        last computed evaluation reuses that evaluation's residual of the remaining blocks; 0 / None: off.  ``per_sample``: one
+        decision per sample instead of one per batch (vcb_flux_set_first_block_cache_ex).  Each ``forward`` then waits for its
+        decision on the host (not capturable in a CUDA graph)."""
         t = first_block_cache_threshold(threshold)
+        per_sample = bool(per_sample)
         if t > 0 and self._sp is not None:
             raise ValueError("the first-block cache decides per batch on one GPU; it is refused with sequence parallelism")
-        check(self.lib.vcb_flux_set_first_block_cache(self._h, t), "vcb_flux_set_first_block_cache")
-        if (t > 0) != (self._fbc > 0):
+        check(self.lib.vcb_flux_set_first_block_cache_ex(self._h, t, int(per_sample)), "vcb_flux_set_first_block_cache_ex")
+        if (t > 0) != (self._fbc > 0) or (t > 0 and per_sample != self._fbc_per_sample):
             self._shape = None                 # the workspace layout changed: prepare again
-        self._fbc = t
+        self._fbc, self._fbc_per_sample = t, per_sample
 
     def cache_stats(self) -> dict:
         """{"computed", "skipped"}: evaluations since the last ``prepare``; "last_diff": the latest evaluation's relative change of
@@ -103,6 +106,15 @@ class FluxEngine:
         c, s, d = C.c_int32(), C.c_int32(), C.c_float()
         check(self.lib.vcb_flux_cache_stats(self._h, C.byref(c), C.byref(s), C.byref(d)), "vcb_flux_cache_stats")
         return {"computed": int(c.value), "skipped": int(s.value), "last_diff": float(d.value)}
+
+    def sample_cache_stats(self) -> list[dict]:
+        """``cache_stats`` of every sample of the prepared batch: its own counters in per-sample mode, the batch's otherwise."""
+        if self._shape is None:
+            raise _lib.VcbError("FluxEngine.sample_cache_stats called before prepare")
+        B = self._shape[0]
+        c, s, d = (C.c_int32 * B)(), (C.c_int32 * B)(), (C.c_float * B)()
+        check(self.lib.vcb_flux_cache_stats_per_sample(self._h, B, c, s, d), "vcb_flux_cache_stats_per_sample")
+        return [{"computed": int(c[b]), "skipped": int(s[b]), "last_diff": float(d[b])} for b in range(B)]
 
     # ---- weight packing -----------------------------------------------------------------------
     def _linear(self, name: str, fp8: bool = False) -> LinearW:

@@ -129,6 +129,7 @@ class Flux(nn.Module):
         self.lora_mode = "merged"
         self._sp = None
         self._fbc = 0.0
+        self._fbc_per_sample = False
         kw = dict(device=device, dtype=dtype)
         for name, fin, fout in linear_table(params):
             _attach(self, name + ".weight", nn.Parameter(torch.empty(fout, fin, **kw), requires_grad=False))
@@ -195,7 +196,7 @@ class Flux(nn.Module):
             if getattr(self, "_sp", None) is not None:
                 self._engine.enable_sequence_parallel(self._sp)
             if self._fbc:
-                self._engine.set_first_block_cache(self._fbc)
+                self._engine.set_first_block_cache(self._fbc, self._fbc_per_sample)
         return self._engine
 
     def set_linear_precision(self, precision: str) -> None:
@@ -238,23 +239,33 @@ class Flux(nn.Module):
         if self._engine is not None:
             self._engine.enable_sequence_parallel(sp)
 
-    def enable_first_block_cache(self, threshold: float | None) -> None:
+    def enable_first_block_cache(self, threshold: float | None, per_sample: bool = False) -> None:
         """Opt-in first-block cache (FBCache; no counterpart in the reference, NOT the reference's numerics).  Within one sampler
         solve, every evaluation runs double block 0; when its img-row residual differs from the one of the last fully computed
         evaluation by less than ``threshold`` (sum|r - r_ref| / sum|r_ref| over the valid rows of the whole batch), the other blocks
         are skipped and their residual from that evaluation is reused.  The first evaluation of a solve is always computed.
         ``None`` or 0 switches it off (the default).  Composes with both LoRA modes and the fp8 precisions; refused with sequence
-        parallelism.  No threshold is recommended: quality on trained weights has not been measured (DESIGN.md §2d)."""
+        parallelism.  No threshold is recommended: quality on trained weights has not been measured (DESIGN.md §2d).
+        ``per_sample``: decide every sample of a batch on its own rows (DESIGN.md §2g), so that a request's output does not depend
+        on the other requests it shares a batched solve with; at batch 1 both modes give the same bits."""
         t = first_block_cache_threshold(threshold)
+        if not isinstance(per_sample, bool):
+            raise ValueError(f"per_sample must be a bool, got {per_sample!r}")
         if t > 0 and self._sp is not None and self._sp.world > 1:
             raise ValueError("the first-block cache decides per batch on one GPU; it is refused with sequence parallelism")
-        self._fbc = t
+        self._fbc, self._fbc_per_sample = t, per_sample
         if self._engine is not None:
-            self._engine.set_first_block_cache(t)
+            self._engine.set_first_block_cache(t, per_sample)
 
-    def cache_stats(self) -> dict:
+    def cache_stats(self, per_sample: bool = False):
         """First-block cache counters of the latest solve (or ``forward``): evaluations "computed" and "skipped" and the latest
-        "last_diff" (inf for the first evaluation of a solve, NaN before any)."""
+        "last_diff" (inf for the first evaluation of a solve, NaN before any).  In per-sample mode an evaluation counts as skipped
+        when every sample skipped, and "last_diff" is the largest sample's.  ``per_sample=True``: a list with those counters for
+        each sample of the latest solve (each sample's own in per-sample mode, the batch's otherwise)."""
+        if per_sample:
+            if self._engine is None or self._engine._shape is None:
+                return []
+            return self._engine.sample_cache_stats()
         if self._engine is None:
             return {"computed": 0, "skipped": 0, "last_diff": math.nan}
         return self._engine.cache_stats()

@@ -24,7 +24,7 @@ import numpy as np
 import torch
 from PIL import Image
 
-from . import ops, resample
+from . import _lib as _vcb_lib, ops, resample
 from .model import FluxLoraWrapper, flux_dev_fill_params
 from .sampling import prepare_modified
 from .transport import Sampler, create_transport
@@ -172,6 +172,67 @@ def run_cell_device(image: torch.Tensor | None, cell: CellPlan, out: torch.Tenso
     ops.u8_to_model_input(im, box or (0, 0, w, h), out, col0)
 
 
+class GridRequest(NamedTuple):
+    """One request of ``VisualClozeModel.process_images_batch``: ``grid`` = (rows, cols), ``images`` / ``prompts`` / ``seed`` /
+    ``cfg`` as ``set_grid_size(*grid)`` followed by ``process_images(images, prompts, seed, cfg)`` takes them."""
+    grid: tuple
+    images: list
+    prompts: list
+    seed: int = 0
+    cfg: float = 30
+
+
+def grid_tokens(cells, grid_h: int, grid_w: int) -> int:
+    """Image tokens Li of a grid laid out by ``grid_plan``: every row is as high as its first cell and as wide as its cells together,
+    one token per 16 x 16 pixels."""
+    return sum(cells[i * grid_w].size[1] // 16 * sum(c.size[0] for c in cells[i * grid_w:(i + 1) * grid_w]) // 16 for i in range(grid_h))
+
+
+def bucket_requests(token_counts, max_batch: int) -> list:
+    """Which requests share a solve: indices with equal image-token counts (equal ``mu``, so equal schedules) go together, at most
+    ``max_batch`` per solve; buckets come in order of their first request, requests keep their order inside a bucket.  Different
+    counts never share a solve (nothing is padded).  Any hashable key works in place of a count (e.g. an image size)."""
+    if isinstance(max_batch, bool) or not isinstance(max_batch, int) or max_batch < 1:
+        raise ValueError(f"max_batch must be an int >= 1, got {max_batch!r}")
+    groups = {}
+    for i, n in enumerate(token_counts):
+        groups.setdefault(n, []).append(i)
+    return [idx[k:k + max_batch] for idx in groups.values() for k in range(0, len(idx), max_batch)]
+
+
+# Default samples per batched solve by image-token count Li: (largest Li, batch), first match wins; beyond the last entry 1.
+# Chosen from tools/bench_batch.py on an H100 (DESIGN.md §2g).
+DEFAULT_MAX_BATCH = ((1152, 4),)
+
+
+def default_max_batch(n_tokens: int) -> int:
+    """The measured default of ``process_images_batch``'s ``max_batch`` for solves of ``n_tokens`` image tokens."""
+    for top, b in DEFAULT_MAX_BATCH:
+        if n_tokens <= top:
+            return b
+    return 1
+
+
+def _sdedit_size(target_size) -> tuple:
+    """(w, h) of the SDEdit solve for an output of ``target_size`` (None = 1024 x 1024): at most 1024 x 1024 pixels, aspect kept,
+    both sides floored to multiples of 16 (visualcloze.py:163-175)."""
+    if target_size is None:
+        target_size = (1024, 1024)
+    if target_size[0] * target_size[1] > 1024 * 1024:
+        ar = target_size[0] / target_size[1]
+        new_h = int((1024 * 1024 / ar) ** 0.5)
+        target_size = (int(new_h * ar), new_h)
+    return (target_size[0] // 16) * 16, (target_size[1] // 16) * 16
+
+
+def _strip_content_prefix(content_prompt: str) -> str:
+    """The content prompt of the SDEdit stage: the grid prompt's lead-in phrases removed (visualcloze.py:156-158)."""
+    for c in _CONTENT_PREFIXES:
+        if content_prompt.startswith(c):
+            content_prompt = content_prompt.replace(c, "")
+    return content_prompt
+
+
 def _load_file(path: str, device) -> dict:
     """safetensors (BFL / diffusers releases) or a torch checkpoint (the LoRA files written by train.py:690-705)."""
     if str(path).endswith(".safetensors"):
@@ -298,11 +359,12 @@ class VisualClozeModel:
         processed = [run_cell_pil(images[k // self.grid_w][k % self.grid_w], c) for k, c in enumerate(cells)]
         return processed, mask_position, upsampling_size
 
-    def _grid_rows(self, images):
+    def _grid_rows(self, images, grid=None):
         """The model input of every grid row built on the device, bit-identical to ``torch.cat([image_transform(c) for c in
         row], dim=2)`` over the cells of ``_prepare_grid``: each RGB image is uploaded once, resampled by libvcb200's Pillow
-        resampler and written straight into its row.  -> (rows: fp32 [3, h, W] on the device, mask_position, upsampling_size)."""
-        grid_h, grid_w = self.grid_h, self.grid_w
+        resampler and written straight into its row.  ``grid``: (rows, cols), default ``set_grid_size``'s.
+        -> (rows: fp32 [3, h, W] on the device, mask_position, upsampling_size)."""
+        grid_h, grid_w = grid or (self.grid_h, self.grid_w)
         sizes = [[None if im is None else im.size for im in row] for row in images]
         cells, mask_position, upsampling_size = grid_plan(sizes, grid_h, grid_w, self.resolution)
         rows = []
@@ -389,16 +451,8 @@ class VisualClozeModel:
 
     def _upsampling(self, tile, box, target_size, cfg, upsampling_steps, upsampling_noise, generator, content_prompt):
         """``upsampling`` of the ``box`` crop of a uint8 [H, W, 3] device image."""
-        for c in _CONTENT_PREFIXES:
-            if content_prompt.startswith(c):
-                content_prompt = content_prompt.replace(c, "")
-        if target_size is None:
-            target_size = (1024, 1024)
-        if target_size[0] * target_size[1] > 1024 * 1024:
-            ar = target_size[0] / target_size[1]
-            new_h = int((1024 * 1024 / ar) ** 0.5)
-            target_size = (int(new_h * ar), new_h)
-        size = ((target_size[0] // 16) * 16, (target_size[1] // 16) * 16)
+        content_prompt = _strip_content_prefix(content_prompt)
+        size = _sdedit_size(target_size)
         image = self._sdedit_resize(tile, box, size)
         if upsampling_noise >= 1.0:
             return Image.fromarray(image.cpu().numpy())
@@ -419,3 +473,164 @@ class VisualClozeModel:
         sample = self.sample_fn(x_t, self.model.forward, kw)[-1][:1]
         tile = self.ae.decode_packed(sample, lh // 2, lw // 2)[0]
         return Image.fromarray(tile.permute(1, 2, 0).cpu().numpy())
+
+    # ---- batched requests ----------------------------------------------------------------------------
+    def _batch_size(self, n_tokens: int, n_evals: int, max_batch) -> int:
+        """Samples per solve of ``n_tokens`` image tokens: ``max_batch`` (default: ``default_max_batch``), lowered until the
+        engine's workspace for that batch fits in free device memory with 2 GiB to spare."""
+        want = default_max_batch(n_tokens) if max_batch is None else max_batch
+        if isinstance(want, bool) or not isinstance(want, int) or want < 1:
+            raise ValueError(f"max_batch must be None or an int >= 1, got {max_batch!r}")
+        if want == 1:
+            return 1
+        eng = self.model.engine()
+        free = torch.cuda.mem_get_info(self.device)[0] + (eng._ws.numel() if eng._ws is not None else 0) - (2 << 30)
+        while want > 1 and eng.lib.vcb_flux_workspace_bytes(eng._h, want, n_tokens, self.max_length, n_evals) > free:
+            want -= 1
+        return want
+
+    def _n_evals(self, steps: int) -> int:
+        from .ops import ODE_STAGES
+        return ODE_STAGES[self.solver] * (int(steps) - 1)
+
+    def _solve_batch(self, noise, prompts, conds, cfgs, sample_fn, blend=None):
+        """One sampler solve of B samples with equal image-token counts: ``noise`` [per sample: list of row noises], ``prompts``
+        [B] str, ``conds`` [B] tensors [1, Li, C], ``cfgs`` [B] guidance.  ``blend`` = (latents [B, Li, 64], s): start from
+        ``noise * (1 - s) + latent * s`` (SDEdit).  -> final latent tokens [B, Li, 64]."""
+        dev, dt = self.device, self.dtype
+        inp = prepare_modified(t5=self._need("t5"), clip=self._need("clip"), img=noise, prompt=list(prompts), proportion_empty_prompts=0.0)
+        x = inp["img"]
+        if blend is not None:
+            x = (x * (1 - blend[1]) + blend[0] * blend[1]).to(dt)
+        kw = dict(txt=inp["txt"], txt_ids=inp["txt_ids"], txt_mask=inp["txt_mask"], y=inp["vec"], img_ids=inp["img_ids"],
+                  img_mask=inp["img_mask"], cond=torch.cat(conds, dim=0),
+                  guidance=torch.tensor([float(c) for c in cfgs], device=dev).to(dt))
+        return sample_fn(x, self.model.forward, kw)[-1][:len(prompts)]
+
+    def _decode_groups(self, items, max_batch: int) -> list:
+        """items: (tokens [Li, 64], h, w) -> uint8 [3, 16h, 16w] per item; equal sizes share ``decode_packed`` calls of up to
+        ``max_batch`` images, fewer when the decoder's workspace for them would not fit in free memory with 2 GiB to spare."""
+        out = [None] * len(items)
+        for size in dict.fromkeys((h, w) for _, h, w in items):
+            idx = [k for k, it in enumerate(items) if it[1:] == size]
+            n = min(max_batch, len(idx))
+            if n > 1 and hasattr(self.ae, "_engine"):
+                lib, hnd = _vcb_lib.lib(), self.ae._engine()
+                free = torch.cuda.mem_get_info(self.device)[0] + (self.ae._ws.numel() if self.ae._ws is not None else 0) - (2 << 30)
+                while n > 1 and lib.vcb_vae_workspace_bytes(hnd, n, *size) > free:
+                    n -= 1
+            for chunk in bucket_requests([size] * len(idx), n):
+                tiles = self.ae.decode_packed(torch.stack([items[idx[k]][0] for k in chunk]), *size)
+                for j, k in enumerate(chunk):
+                    out[idx[k]] = tiles[j]
+        return out
+
+    @torch.no_grad()
+    def process_images_batch(self, requests, *, steps: int = 30, upsampling_steps: int = 10, upsampling_noise: float = 0.4,
+                             is_upsampling: bool = True, max_batch: int | None = None) -> list:
+        """Several grids in batched solves.  ``requests``: ``GridRequest``s (or dicts of their fields).  Returns one list of PIL
+        images per request, each what ``set_grid_size(*grid)`` followed by ``process_images(images, prompts, seed, cfg, steps,
+        upsampling_steps, upsampling_noise, is_upsampling)`` returns (within the bf16 batch-invariance of the kernels).
+
+        Requests with the same image-token count share one solve of up to ``max_batch`` samples (None: ``default_max_batch``,
+        lowered to what device memory holds); different counts run apart, nothing is padded.  Every request draws its noise from
+        its own ``torch.Generator(device).manual_seed(seed)`` in the solo order (grid rows, then one SDEdit noise per target in
+        column order); ``seed == 0`` draws a random seed per request.  SDEdit targets of all requests are batched by their own
+        token count.  With the first-block cache on, batched solves decide per sample.  ``set_grid_size`` is left as it was."""
+        reqs = [r if isinstance(r, GridRequest) else GridRequest(**r) for r in requests]
+        dev, dt = self.device, self.dtype
+        fbc, fbc_per_sample = getattr(self.model, "_fbc", 0.0), getattr(self.model, "_fbc_per_sample", False)
+        if fbc > 0 and not fbc_per_sample:
+            self.model.enable_first_block_cache(fbc, per_sample=True)
+        try:
+            return self._process_batch(reqs, int(steps), int(upsampling_steps), float(upsampling_noise), is_upsampling, max_batch, dev, dt)
+        finally:
+            if fbc > 0 and not fbc_per_sample:
+                self.model.enable_first_block_cache(fbc, per_sample=False)
+
+    def _process_batch(self, reqs, steps, upsampling_steps, upsampling_noise, is_upsampling, max_batch, dev, dt):
+        preps = []
+        for r in reqs:
+            grid_h, grid_w = (int(v) for v in r.grid)
+            seed = r.seed if r.seed != 0 else random.randint(0, 2 ** 32 - 1)
+            images = [[im.convert("RGB") if im is not None else None for im in row] for row in r.images]
+            rows, mask_position, upsampling_size = self._grid_rows(images, (grid_h, grid_w))
+            fill_mask = []
+            for i, row in enumerate(rows):
+                h, w = row.shape[1], row.shape[2] // grid_w
+                marks = mask_position if i == grid_h - 1 else [0] * grid_w
+                fill_mask.append(torch.cat([torch.full((1, 1, h, w), float(m), device=dev) for m in marks], dim=3))
+            fill_cond = torch.cat([self._encode_tokens(row) for row in rows], dim=1)
+            fill_mask = torch.cat([_pack_mask(m) for m in fill_mask], dim=1).to(dt)
+            rng = torch.Generator(device=dev).manual_seed(int(seed))
+            sizes = [tuple(row.shape[-2:]) for row in rows]
+            noise = [torch.randn([1, 16, h // 8, w // 8], device=dev, generator=rng).to(dt) for h, w in sizes]
+            preps.append(dict(grid_w=grid_w, mask_position=mask_position, upsampling_size=upsampling_size, rng=rng, sizes=sizes,
+                              noise=noise, cond=torch.cat((fill_cond, fill_mask), dim=-1), Li=sum(h * w // 256 for h, w in sizes)))
+
+        # grid solves: one per bucket of equal Li
+        n_evals = self._n_evals(steps)
+        samples = [None] * len(reqs)
+        for Li in dict.fromkeys(p["Li"] for p in preps):
+            idx = [k for k, p in enumerate(preps) if p["Li"] == Li]
+            for bucket in bucket_requests([Li] * len(idx), self._batch_size(Li, n_evals, max_batch)):
+                ks = [idx[k] for k in bucket]
+                out = self._solve_batch([preps[k]["noise"] for k in ks], [" ".join(reqs[k].prompts) for k in ks],
+                                        [preps[k]["cond"] for k in ks], [reqs[k].cfg for k in ks],
+                                        self._make_sample_fn(steps, True, self.time_shifting_factor, None))
+                for n, k in enumerate(ks):
+                    samples[k] = out[n]
+
+        # decode the query rows, equal sizes together
+        items = []
+        for p, smp in zip(preps, samples):
+            qh, qw = p["sizes"][-1]
+            start = sum(h * w // 256 for h, w in p["sizes"][:-1])
+            items.append((smp[start:start + qh * qw // 256], qh // 16, qw // 16))
+        tiles = self._decode_groups(items, self._batch_size(max(p["Li"] for p in preps), n_evals, max_batch))
+        tiles = [t.permute(1, 2, 0).contiguous() for t in tiles]                                  # uint8 [H, W, 3]
+
+        results, targets = [[] for _ in reqs], []
+        for k, (p, tile) in enumerate(zip(preps, tiles)):
+            ret_h, ret_w = tile.shape[0], tile.shape[1]
+            query = None if is_upsampling else Image.fromarray(tile.cpu().numpy())
+            for j in range(p["grid_w"]):
+                if not p["mask_position"][j]:
+                    continue
+                box = (j * ret_w // p["grid_w"], 0, (j + 1) * ret_w // p["grid_w"], ret_h)
+                if not is_upsampling:
+                    results[k].append(query.crop(box))
+                    continue
+                size = _sdedit_size(p["upsampling_size"])
+                image = self._sdedit_resize(tile, box, size)
+                if upsampling_noise >= 1.0:
+                    results[k].append(Image.fromarray(image.cpu().numpy()))
+                    continue
+                x = ops.u8_to_model_input(image, (0, 0) + size, torch.empty(3, size[1], size[0], dtype=torch.float32, device=dev), 0)
+                latent = self._encode_tokens(x)
+                blank = self._encode_tokens(torch.zeros_like(x))
+                mask = _pack_mask(torch.ones(1, 1, x.shape[1], x.shape[2], device=dev, dtype=dt))
+                noise = torch.randn([1, 16, x.shape[1] // 8, x.shape[2] // 8], device=dev, generator=p["rng"]).to(dt)
+                results[k].append(None)
+                targets.append(dict(req=k, slot=len(results[k]) - 1, size=size, latent=latent, cond=torch.cat((blank, mask), dim=-1),
+                                    noise=noise, cfg=reqs[k].cfg, prompt=_strip_content_prefix(reqs[k].prompts[2])))
+        if not targets:
+            return results
+
+        # SDEdit solves: targets batched by their own token count
+        n_evals = self._n_evals(upsampling_steps)
+        lats = [None] * len(targets)
+        for Li in dict.fromkeys(t["size"][0] * t["size"][1] // 256 for t in targets):
+            idx = [k for k, t in enumerate(targets) if t["size"][0] * t["size"][1] // 256 == Li]
+            for bucket in bucket_requests([Li] * len(idx), self._batch_size(Li, n_evals, max_batch)):
+                ts = [targets[idx[k]] for k in bucket]
+                out = self._solve_batch([[t["noise"]] for t in ts], [t["prompt"] for t in ts], [t["cond"] for t in ts],
+                                        [t["cfg"] for t in ts], self._make_sample_fn(upsampling_steps, False, 1.0, upsampling_noise),
+                                        blend=(torch.cat([t["latent"] for t in ts], dim=0), upsampling_noise))
+                for n, k in enumerate(bucket):
+                    lats[idx[k]] = out[n]
+        tiles = self._decode_groups([(lat, t["size"][1] // 16, t["size"][0] // 16) for lat, t in zip(lats, targets)],
+                                    self._batch_size(max(t["size"][0] * t["size"][1] // 256 for t in targets), n_evals, max_batch))
+        for t, tile in zip(targets, tiles):
+            results[t["req"]][t["slot"]] = Image.fromarray(tile.permute(1, 2, 0).cpu().numpy())
+        return results
